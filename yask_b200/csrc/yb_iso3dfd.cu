@@ -133,7 +133,7 @@ EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// 3-D tiled map over one step slot of a var (dims x,y,z; z unit stride) with box (bz, by, 1).
+// 3-D tiled map over one step slot of a var (dims x,y,z; z unit stride) with box (bz, by, 1); FLOAT32 or FLOAT64 elements.
 int make_map(CUtensorMap* map, const Var& v, int slot, int bz, int by) {
     EncodeTiledFn enc = get_encode_fn();
     if (!enc) return set_error(YB_ECUDA, "cuTensorMapEncodeTiled not available from the driver");
@@ -141,10 +141,11 @@ int make_map(CUtensorMap* map, const Var& v, int slot, int bz, int by) {
     const Dim* dy = v.domain_dim(1);
     const Dim* dz = v.domain_dim(2);
     cuuint64_t gdim[3] = {cuuint64_t(dz->alloc), cuuint64_t(dy->alloc), cuuint64_t(dx->alloc)};
-    cuuint64_t gstr[2] = {cuuint64_t(dy->stride) * 4, cuuint64_t(dx->stride) * 4};
+    const cuuint64_t eb = cuuint64_t(v.elem_bytes);
+    cuuint64_t gstr[2] = {cuuint64_t(dy->stride) * eb, cuuint64_t(dx->stride) * eb};
     cuuint32_t box[3] = {cuuint32_t(bz), cuuint32_t(by), 1};
     cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, v.slot_ptr(slot), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = enc(map, v.elem_bytes == 8 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT64 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, v.slot_ptr(slot), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(YB_ECUDA, "cuTensorMapEncodeTiled failed with code %d", int(r));
     return 0;
@@ -244,6 +245,7 @@ __global__ void slot_box_copy_kernel(float* dst, const float* src, long long sx,
 
 struct IsoEngine : Engine {
     int radius = 8;
+    bool f64 = false;              // 8-byte elements: the double-precision sweep (iso_radius_cfg_f64), one compiled variant per radius
     double coef[ISO_MAX_R + 1] = {0};
     std::string kernel = "auto";   // auto | tma | direct
     int tile = DEFAULT_TILE;       // index into tile_cfg(): 16x128, producer warpgroup, 2 planes per trip
@@ -327,7 +329,10 @@ struct IsoEngine : Engine {
     int prepare(Solution& s) override {
         radius = s.spec.radius;
         if (radius < 1 || radius > ISO_MAX_R) return set_error(YB_EUNSUPPORTED, "iso3dfd radius must be in 1..%d", ISO_MAX_R);
-        if (s.spec.elem_bytes != 4) return set_error(YB_EUNSUPPORTED, "iso3dfd: only 4-byte elements are implemented in this round");
+        if (s.spec.elem_bytes != 4 && s.spec.elem_bytes != 8) return set_error(YB_EUNSUPPORTED, "iso3dfd: elements must be 4 or 8 bytes");
+        f64 = s.spec.elem_bytes == 8;
+        if (f64 && !iso_radius_cfg_f64(radius))
+            return set_error(YB_EUNSUPPORTED, "iso3dfd fp64: the hand-written sweep serves radius 1, 2, 4, 5, 6 and 7 (3 and 8 are generated)");
         iso3dfd_coeffs(radius, coef);
         cudaDeviceProp prop;
         YB_CUDA(cudaGetDeviceProperties(&prop, s.device));
@@ -336,18 +341,19 @@ struct IsoEngine : Engine {
         tt_ok = false;
         const int nsl = s.vars[0].nslots();
         if (nsl > 4) return set_error(YB_EUNSUPPORTED, "iso3dfd: at most 4 storage slots of p");
-        if (prop.major >= 9 && (radius == 8 || iso_radius_cfg(radius))) {
+        if (prop.major >= 9 && f64) {
+            const TileCfgT<double>& c = *iso_radius_cfg_f64(radius);
+            for (int cur = 0; cur < nsl; cur++)
+                if (int rc = make_maps(s, c, cur, maps[0][cur])) return rc;
+            maps_ok = true;
+            for (int m = 0; m < 3; m++) preload_kernel((const void*)c.fn[m]);
+        } else if (prop.major >= 9 && (radius == 8 || iso_radius_cfg(radius))) {
             const Var& p = s.vars[0];
             const Var& v = s.vars[1];
             for (int tl = 0; tl < (radius == 8 ? NTILES : 1); tl++) {
                 const TileCfg& c = radius == 8 ? tile_cfg(tl) : *iso_radius_cfg(radius);
-                for (int cur = 0; cur < nsl; cur++) {
-                    IsoMaps& m = maps[tl][cur];
-                    if (int rc = make_map(&m.h, p, cur, c.hp, c.hrows)) return rc;
-                    if (int rc = make_map(&m.c, p, cur, c.tz, c.ty)) return rc;
-                    if (int rc = make_map(&m.p, p, cur ^ 1, c.tz, c.ty)) return rc;
-                    if (int rc = make_map(&m.v, v, 0, c.tz, c.ty)) return rc;
-                }
+                for (int cur = 0; cur < nsl; cur++)
+                    if (int rc = make_maps(s, c, cur, maps[tl][cur])) return rc;
             }
             maps_ok = true;
             if (const TTCfg* tc = (p.extra_slots == 2 && nsl == 4) ? tt_radius_cfg(radius, 0) : nullptr) {
@@ -365,23 +371,48 @@ struct IsoEngine : Engine {
             const TileCfg& c = radius == 8 ? tile_cfg(tile) : *iso_radius_cfg(radius);
             for (int m = 0; m < 4; m++) preload_kernel((const void*)c.fn[m]);
         }
-        preload_kernel((const void*)iso3dfd_direct_kernel<0>);
-        preload_kernel((const void*)iso3dfd_direct_kernel<1>);
-        preload_kernel((const void*)iso3dfd_direct_kernel<2>);
+        if (f64) {
+            preload_kernel((const void*)iso3dfd_direct_kernel<double, 0>);
+            preload_kernel((const void*)iso3dfd_direct_kernel<double, 1>);
+            preload_kernel((const void*)iso3dfd_direct_kernel<double, 2>);
+        } else {
+            preload_kernel((const void*)iso3dfd_direct_kernel<float, 0>);
+            preload_kernel((const void*)iso3dfd_direct_kernel<float, 1>);
+            preload_kernel((const void*)iso3dfd_direct_kernel<float, 2>);
+        }
         return 0;
     }
 
-    void fill_params(const Solution& s, int64_t t, const Box& box, IsoParams& P) const {
+    // Tensor maps of one sweep variant with p(t) in slot `cur`.
+    template <class E>
+    static int make_maps(const Solution& s, const TileCfgT<E>& c, int cur, IsoMaps& m) {
+        const Var& p = s.vars[0];
+        const Var& v = s.vars[1];
+        if (int rc = make_map(&m.h, p, cur, c.hp, c.hrows)) return rc;
+        if (int rc = make_map(&m.c, p, cur, c.tz, c.ty)) return rc;
+        if (int rc = make_map(&m.p, p, cur ^ 1, c.tz, c.ty)) return rc;
+        return make_map(&m.v, v, 0, c.tz, c.ty);
+    }
+
+    // The sweep variant a launch uses: the selected tile at radius 8, the one compiled variant at other radii.
+    template <class E>
+    const TileCfgT<E>& sweep_cfg() const {
+        if constexpr (sizeof(E) == 8) return *iso_radius_cfg_f64(radius);
+        else return radius == 8 ? tile_cfg(tile) : *iso_radius_cfg(radius);
+    }
+
+    template <class E>
+    void fill_params(const Solution& s, int64_t t, const Box& box, IsoParamsT<E>& P) const {
         const Var& p = s.vars[0];
         const Var& v = s.vars[1];
         const int cur = p.slot_of(t);
         const Dim *px = p.domain_dim(0), *py = p.domain_dim(1), *pz = p.domain_dim(2);
         const Dim *vx = v.domain_dim(0), *vy = v.domain_dim(1), *vz = v.domain_dim(2);
         // p(t+1) is written over p(t-1) (/root/reference/src/compiler/lib/Var.cpp:435-464): slot_of(t+1) == slot_of(t-1)
-        P.out = reinterpret_cast<float*>(p.slot_ptr(p.slot_of(t + 1))) + p.origin_offset();
-        P.prev = reinterpret_cast<const float*>(p.slot_ptr(p.slot_of(t - 1))) + p.origin_offset();
-        P.cur = reinterpret_cast<const float*>(p.slot_ptr(cur)) + p.origin_offset();
-        P.vel = reinterpret_cast<const float*>(v.slot_ptr(0)) + v.origin_offset();
+        P.out = reinterpret_cast<E*>(p.slot_ptr(p.slot_of(t + 1))) + p.origin_offset();
+        P.prev = reinterpret_cast<const E*>(p.slot_ptr(p.slot_of(t - 1))) + p.origin_offset();
+        P.cur = reinterpret_cast<const E*>(p.slot_ptr(cur)) + p.origin_offset();
+        P.vel = reinterpret_cast<const E*>(v.slot_ptr(0)) + v.origin_offset();
         P.out_sx = px->stride; P.out_sy = py->stride;
         P.v_sx = vx->stride; P.v_sy = vy->stride;
         P.nx = int(px->domain); P.ny = int(py->domain); P.nz = int(pz->domain);
@@ -391,14 +422,19 @@ struct IsoEngine : Engine {
         P.pad_x = int(px->pad_l); P.pad_y = int(py->pad_l); P.pad_z = int(pz->pad_l);
         P.vpad_x = int(vx->pad_l); P.vpad_y = int(vy->pad_l); P.vpad_z = int(vz->pad_l);
         P.pol_c = pol_c; P.pol_h = pol_h; P.pol_pv = pol_pv; P.st_cs = st_cs; P.peer_probe = peer_probe;
-        for (int r = 0; r <= ISO_MAX_R; r++) P.c[r] = r <= radius ? float(coef[r]) : 0.f;
+        for (int r = 0; r <= ISO_MAX_R; r++) P.c[r] = r <= radius ? E(coef[r]) : E(0);    // fp64: the round-tripped doubles as they are
     }
 
     int launch(Solution& s, int, int64_t t, const Box& box, cudaStream_t st) override {
         if (box.empty()) return 0;
+        return f64 ? launch_sweep<double>(s, t, box, st) : launch_sweep<float>(s, t, box, st);
+    }
+
+    template <class E>
+    int launch_sweep(Solution& s, int64_t t, const Box& box, cudaStream_t st) {
         const Var& p = s.vars[0];
         const int cur = p.slot_of(t);
-        IsoParams P{};
+        IsoParamsT<E> P{};
         fill_params(s, t, box, P);
         int mode = s.fp_mode;
         bool use_tma = maps_ok && kernel != "direct";
@@ -408,8 +444,8 @@ struct IsoEngine : Engine {
         }
         if (kernel == "tma" && !maps_ok) return set_error(YB_EUNSUPPORTED, "the tiled TMA kernel needs sm_90+");
         if (use_tma) {
-            const int ti = radius == 8 ? tile : 0;      // other radii: one compiled variant
-            const TileCfg& c = radius == 8 ? tile_cfg(tile) : *iso_radius_cfg(radius);
+            const int ti = radius == 8 ? tile : 0;      // other radii and fp64: one compiled variant
+            const TileCfgT<E>& c = sweep_cfg<E>();
             if (mem_probe && c.fn[3]) mode = 3;
             // fused halo exchange: only for whole-domain launches of a kernel that implements the peer stores
             P.peer_lo = P.peer_hi = nullptr;
@@ -420,8 +456,8 @@ struct IsoEngine : Engine {
             const bool nb_lo = fused && s.fused_x.lo != nullptr, nb_hi = fused && s.fused_x.hi != nullptr;   // x neighbours
             if (fused) {
                 if (!s.fused_x.dma) {        // the kernel stores the boundary planes into the neighbours itself
-                    P.peer_lo = static_cast<float*>(s.fused_x.lo);
-                    P.peer_hi = static_cast<float*>(s.fused_x.hi);
+                    P.peer_lo = static_cast<E*>(s.fused_x.lo);
+                    P.peer_hi = static_cast<E*>(s.fused_x.hi);
                 }
                 s.fused_x.used = true;
             }
@@ -472,7 +508,7 @@ struct IsoEngine : Engine {
             int grid = int(std::min<int64_t>(nunits, gmax));
             if (sig) {
                 P.sig_units = int(ntile) * nsig;
-                P.sig_total = unsigned(grid) * unsigned(c.ty * c.tz / 8 / 32);     // consumer warps: 8 points per thread
+                P.sig_total = unsigned(grid) * unsigned(c.ty * c.tz / (2 * IsoVec<E>::N) / 32);   // consumer warps: 2 vectors per thread
                 P.sig_counter = s.fused_x.counter;
                 P.sig_flag_lo = s.fused_x.flag_lo; P.sig_flag_hi = s.fused_x.flag_hi;
                 P.sig_epoch = s.fused_x.epoch;
@@ -488,9 +524,9 @@ struct IsoEngine : Engine {
             dim3 grd(unsigned((box.e[2] - box.b[2] + 127) / 128), unsigned(box.e[1] - box.b[1]), unsigned(box.e[0] - box.b[0]));
             if (grd.y > 65535 || grd.z > 65535) return set_error(YB_EUNSUPPORTED, "direct kernel: domain too large in x or y");
             switch (mode) {
-                case 0: iso3dfd_direct_kernel<0><<<grd, blk, 0, st>>>(P, radius); break;
-                case 1: iso3dfd_direct_kernel<1><<<grd, blk, 0, st>>>(P, radius); break;
-                default: iso3dfd_direct_kernel<2><<<grd, blk, 0, st>>>(P, radius); break;
+                case 0: iso3dfd_direct_kernel<E, 0><<<grd, blk, 0, st>>>(P, radius); break;
+                case 1: iso3dfd_direct_kernel<E, 1><<<grd, blk, 0, st>>>(P, radius); break;
+                default: iso3dfd_direct_kernel<E, 2><<<grd, blk, 0, st>>>(P, radius); break;
             }
         }
         YB_CUDA(cudaGetLastError());
@@ -645,15 +681,16 @@ struct IsoEngine : Engine {
 
     // Offline tuner: the compiled sweep variants (tile shape, producer warpgroup, planes per trip) x sweep chunk
     // lengths, timed over the whole rank box; the analogue of the reference's block-size search
-    // (/root/reference/src/kernel/lib/auto_tuner.cpp) for the knobs this engine has.
+    // (/root/reference/src/kernel/lib/auto_tuner.cpp) for the knobs this engine has.  fp64 has one variant per radius: only
+    // the chunk length is searched.
     int auto_tune(Solution& s, cudaStream_t st, std::string& report) override {
         if (tt_ok && kernel != "direct" && !s.multi_rank()) return auto_tune_temporal(s, st, report);
-        if (!maps_ok || radius != 8 || kernel == "direct") { report = "iso3dfd: no tiled variants to tune for this configuration"; return 0; }
+        if (!maps_ok || (radius != 8 && !f64) || kernel == "direct") { report = "iso3dfd: no tiled variants to tune for this configuration"; return 0; }
         Box whole;
         for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = s.rank_size[d]; }
         if (whole.e[1] < 8 || whole.e[2] < 16) { report = "iso3dfd: domain too thin for the tiled kernel"; return 0; }
         const int64_t t0 = s.vars[0].last_valid_step();
-        const int tiles[] = {7, 6, 5, 4, 1, 0};
+        const std::vector<int> tiles = f64 ? std::vector<int>{tile} : std::vector<int>{7, 6, 5, 4, 1, 0};
         const int lxs[] = {0, 256, 512, 1024};   // planes per interior chunk (0 = cost model)
         const int keep_tile = tile, keep_lx = lx;
         double best = 1e30;
@@ -667,7 +704,7 @@ struct IsoEngine : Engine {
                 int64_t t = t0;
                 const double ms = time_launches(st, 3, [&]() { return launch(s, 0, t++, whole, st); });
                 if (ms < 0) { tile = keep_tile; lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-                snprintf(line, sizeof line, " tile=%d (%s) lx=%d: %.4f ms/step\n", ti, tile_cfg(ti).name, l, ms);
+                snprintf(line, sizeof line, " tile=%d (%s) lx=%d: %.4f ms/step\n", ti, f64 ? iso_radius_cfg_f64(radius)->name : tile_cfg(ti).name, l, ms);
                 report += line;
                 if (ms < best) { best = ms; best_tile = ti; best_lx = l; }
             }

@@ -11,6 +11,9 @@
 //
 // FP modes (see oracle/yask_oracle.c): 0 strict IEEE mul/add, 1 canonical FMA,
 // 2 = FMA pattern GCC 13 emits for the reference's default build (bit-exact vs it).
+//
+// Every kernel here is written for an element type E, float or double (the reference's real_bytes=4 / 8).  A thread
+// moves 16-byte vectors: 4 floats (float4) or 2 doubles (double2).
 #pragma once
 #include <type_traits>
 
@@ -22,12 +25,18 @@ namespace yb {
 constexpr int ISO_MAX_R = 8;
 constexpr int ISO_MAX_CHUNKS = 40;   // x chunks of one launch (boundary chunks + interior chunks)
 
-struct IsoParams {
-    float* out;             // &p_next[domain origin]; written in place over p(t-1)
+// 16-byte vector of the element type: the unit of shared-memory loads, x-queue entries and global stores.
+template <class E> struct IsoVec;
+template <> struct IsoVec<float> { using V = float4; static constexpr int N = 4; };
+template <> struct IsoVec<double> { using V = double2; static constexpr int N = 2; };
+
+template <class E>
+struct IsoParamsT {
+    E* out;             // &p_next[domain origin]; written in place over p(t-1)
     long long out_sx, out_sy;  // element strides of the p arrays (z stride is 1)
-    const float* cur;       // &p_cur[domain origin]  (naive kernel only)
-    const float* prev;      // &p_prev[domain origin] (naive kernel only): == out unless the var has extra storage slots
-    const float* vel;       // &v[domain origin]      (naive kernel only)
+    const E* cur;           // &p_cur[domain origin]  (naive kernel only)
+    const E* prev;          // &p_prev[domain origin] (naive kernel only): == out unless the var has extra storage slots
+    const E* vel;           // &v[domain origin]      (naive kernel only)
     long long v_sx, v_sy;
     int nx, ny, nz;         // rank-domain sizes
     int x_begin, x_end;     // sub-range of x planes to compute (boundary/interior split)
@@ -48,8 +57,8 @@ struct IsoParams {
                                 // 2 = CTAs start a few microseconds apart so that their boundary phases do not coincide
     // Fused halo exchange: when non-null, the first / last R computed x planes are ALSO stored into the lower /
     // upper x neighbour's halo cells (peer HBM over NVLink), indexed exactly like `out`.
-    float* peer_lo;
-    float* peer_hi;
+    E* peer_lo;
+    E* peer_hi;
     // In-kernel completion signal of the boundary planes (replaces the push + signal kernels that used to follow the
     // sweep): units [0, sig_units) are the units whose sweeps START with boundary planes.  Every consumer warp of the
     // grid arrives once on *sig_counter, right after the R-th plane of its last such unit (system-scope fence first);
@@ -63,29 +72,30 @@ struct IsoParams {
     unsigned long long* sig_flag_lo;
     unsigned long long* sig_flag_hi;
     unsigned long long sig_epoch;
-    float c[ISO_MAX_R + 1];
+    E c[ISO_MAX_R + 1];
 };
+using IsoParams = IsoParamsT<float>;
 
 // ---------------------------------------------------------------------------------------------
 // Reference-order direct kernel: one thread per point, straight global loads (through L1/L2).
 // Used for radii/shapes the tiled kernel does not cover and as the on-device cross-check of the
 // tiled kernel at sizes the CPU oracle cannot reach.  Any radius 1..8.
 // ---------------------------------------------------------------------------------------------
-template <int MODE>
-__global__ void __launch_bounds__(256) iso3dfd_direct_kernel(IsoParams P, int R) {
+template <class E, int MODE>
+__global__ void __launch_bounds__(256) iso3dfd_direct_kernel(IsoParamsT<E> P, int R) {
     const int z = P.z_begin + blockIdx.x * blockDim.x + threadIdx.x;
     const int y = P.y_begin + blockIdx.y;
     const int x = P.x_begin + blockIdx.z;
     if (z >= P.z_end || y >= P.y_end || x >= P.x_end) return;
     const long long o = (long long)x * P.out_sx + (long long)y * P.out_sy + z;
-    const float* pc = P.cur + o;
-    const float center = pc[0];
-    float acc = 0.f;
+    const E* pc = P.cur + o;
+    const E center = pc[0];
+    E acc = 0;
     for (int r = 1; r <= R; r++) {
         acc = iso_group<MODE>(acc, center, P.c[0], P.c[r], pc[-r * P.out_sx], pc[r * P.out_sx], pc[-r * P.out_sy],
                               pc[r * P.out_sy], pc[-r], pc[r], r == 1);
     }
-    const float v = P.vel[(long long)x * P.v_sx + (long long)y * P.v_sy + z];
+    const E v = P.vel[(long long)x * P.v_sx + (long long)y * P.v_sy + z];
     P.out[o] = iso_final<MODE>(acc, center, P.prev[o], v);
 }
 
@@ -97,7 +107,7 @@ __global__ void __launch_bounds__(256) iso3dfd_direct_kernel(IsoParams P, int R)
 // z-consecutive points for every plane of the sweep.
 //
 //   * x neighbours: a 2R+1 deep register queue of the thread's own quads, rotated by register moves.
-//   * y,z neighbours: the current plane with halo, (TY+2R) x (TZ+2HZ) floats, staged in shared
+//   * y,z neighbours: the current plane with halo, (TY+2R) x (TZ+2HZ) elements, staged in shared
 //     memory by ONE TMA box load (cp.async.bulk.tensor.3d, box depth 1).
 //   * the queue is fed by a second, halo-less TMA box R planes ahead of the current one;
 //     p(t-1) and v tiles arrive the same way (evict-first: they are streamed exactly once).
@@ -127,8 +137,8 @@ struct IsoCursor {
     uint32_t phase;
 };
 
-template <class T>
-__device__ __forceinline__ void iso_unit_setup(IsoCursor& cu, const IsoParams& P) {
+template <class T, class PT>
+__device__ __forceinline__ void iso_unit_setup(IsoCursor& cu, const PT& P) {
     int u = cu.unit;
     const int tz = u % P.ntz; u /= P.ntz;
     const int ty = u % P.nty; u /= P.nty;
@@ -145,26 +155,36 @@ __device__ __forceinline__ void iso_unit_setup(IsoCursor& cu, const IsoParams& P
 //
 // The first version of this kernel (one row x 4 z per thread, sweep loop unrolled 2R+1 times) was limited by shared-memory wavefronts (23 LDS.128 per 4 points,
 // every y neighbour loaded once per point) and by instruction-cache misses of the unrolled body.  Hence:
-//   * a thread owns TWO vertically adjacent rows x 4 z (8 points).  The y window of the pair is
+//   * a thread owns TWO vertically adjacent rows x 4 z (8 points; 2 z and 4 points in fp64).  The y window of the pair is
 //     18 rows, each loaded ONCE and used by both rows: 16+8 neighbour loads per 8 points
 //     instead of 2 x 20 -- 40 % fewer shared-memory wavefronts per point;
 //   * the x queue is rotated by register moves (loop NOT unrolled 2R+1 times), so the whole
 //     sweep body fits the instruction cache.
 // ---------------------------------------------------------------------------------------------
-template <int R_, int TYP_, int TZQ_, int STAGES_>
+// E = double: a thread's rows are one double2 wide, so the same thread layout covers half the z extent (TZ = 2 * TZQ)
+// with the same registers per x-queue entry, and the z halo rounds up to whole double2 vectors.
+template <int R_, int TYP_, int TZQ_, int STAGES_, class E_ = float>
 struct IsoTile2 {
+    using E = E_;
+    using V = typename IsoVec<E>::V;
+    static constexpr int VW = IsoVec<E>::N;     // elements per 16-byte vector
+    static constexpr int ES = int(sizeof(E));
     static constexpr int R = R_, TYP = TYP_, TZQ = TZQ_, STAGES = STAGES_;
     static constexpr int TY = 2 * TYP;
-    static constexpr int TZ = 4 * TZQ;
-    static constexpr int HZ = (R + 3) / 4 * 4;
-    static constexpr int ZQ = HZ / 4;
+    static constexpr int TZ = VW * TZQ;
+    static constexpr int HZ = (R + VW - 1) / VW * VW;
+    static constexpr int ZQ = HZ / VW;
     static constexpr int HP = TZ + 2 * HZ;
     static constexpr int HROWS = TY + 2 * R;
     static constexpr int THREADS = TYP * TZQ;
     static constexpr int NWARPS = THREADS / 32;
     static constexpr int QN = 2 * R + 1;
-    static constexpr uint32_t H_BYTES = HROWS * HP * 4;
-    static constexpr uint32_t C_BYTES = TY * TZ * 4;
+    // setmaxnreg split of a CTA with a producer warpgroup (128 x PROD_REGS + THREADS x CONS_REGS <= 64K registers).  The fp64
+    // producer keeps twice the fp32 budget: its unit bookkeeping then stays in registers (24 spill a few bytes to the stack).
+    static constexpr int PROD_REGS = sizeof(E) == 8 ? 48 : 24;
+    static constexpr int CONS_REGS = sizeof(E) == 8 ? 224 : 240;
+    static constexpr uint32_t H_BYTES = HROWS * HP * ES;
+    static constexpr uint32_t C_BYTES = TY * TZ * ES;
     static constexpr uint32_t H_OFF = 0;
     static constexpr uint32_t C_OFF = (H_BYTES + 127) / 128 * 128;
     static constexpr uint32_t P_OFF = C_OFF + C_BYTES;
@@ -177,7 +197,8 @@ struct IsoTile2 {
 };
 
 // Boundary-phase completion (see IsoParams::sig_*): called once per consumer warp, by all of its lanes.
-static __device__ __noinline__ void iso_boundary_arrive(const IsoParams& P, int lane) {
+template <class PT>
+__device__ __noinline__ void iso_boundary_arrive(const PT& P, int lane) {
     __threadfence_system();          // this lane's peer stores are ordered before what follows, at system scope
     __syncwarp();
     if (lane == 0) {
@@ -192,6 +213,9 @@ static __device__ __noinline__ void iso_boundary_arrive(const IsoParams& P, int 
 }
 
 __device__ __forceinline__ void f4_to_arr(const float4& v, float* a) { a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w; }
+__device__ __forceinline__ void f4_to_arr(const double2& v, double* a) { a[0] = v.x; a[1] = v.y; }
+__device__ __forceinline__ void arr_to_v(const float* a, float4& v) { v = make_float4(a[0], a[1], a[2], a[3]); }
+__device__ __forceinline__ void arr_to_v(const double* a, double2& v) { v = make_double2(a[0], a[1]); }
 
 // PW = 1: a dedicated producer warp (warp NWARPS) issues the TMA loads, so no compute warp carries the
 //         issue code (with 2 warps per scheduler a straggling warp 0 delays every stage hand-over).
@@ -199,9 +223,14 @@ __device__ __forceinline__ void f4_to_arr(const float4& v, float* a) { a[0] = v.
 //         plane (half the register moves of U = 1) at the price of one extra queue entry per row.
 template <class T, int MODE, int PW = 0, int U = 1>
 __global__ void __launch_bounds__(T::THREADS + 128 * PW, 1)
-iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ IsoParams P) {
-    constexpr int R = T::R, QN = T::QN, ZQ = T::ZQ;
+iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ IsoParamsT<typename T::E> P) {
+    using E = typename T::E;
+    using V = typename T::V;
+    constexpr int R = T::R, QN = T::QN, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
     constexpr int QL = QN + (U - 1);          // queue entries kept per row
+    // The fused halo exchange (peer stores + completion signal) is compiled for fp32 only: the fp64 sweep is listed with
+    // fused_ok = false, and leaving the out-of-line signal call out keeps its registers free of call spills.
+    constexpr bool FUSED = sizeof(E) == 4;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     uint8_t* sbase = smem_raw + (base - smem_u32(smem_raw));
@@ -251,11 +280,11 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
         // Warp-specialised register budget (setmaxnreg works on whole warpgroups): the producer warpgroup
         // hands its registers back, the two consumer warpgroups take them.
         if (tid >= T::THREADS) {          // producer warpgroup: one lane streams every load of this CTA, then exits
-            asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+            asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T::PROD_REGS));
             while (pr_live) produce_one();
             return;
         }
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T::CONS_REGS));
     } else if (tid == 0) {
         for (int k = 0; k < T::STAGES - 1 && pr_live; k++) produce_one();
     }
@@ -264,25 +293,25 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
     // ---- consumer ------------------------------------------------------------------------------------
     const int rp = tid / T::TZQ;           // row pair 0..TYP-1  (rows 2rp, 2rp+1)
     const int quad = tid % T::TZQ;
-    const uint32_t h_own = ((2 * rp + R) * T::HP + T::HZ + 4 * quad) * 4;  // row a centre in H
-    const uint32_t c_own = (2 * rp * T::TZ + 4 * quad) * 4;               // row a in C/P/V tiles
+    const uint32_t h_own = ((2 * rp + R) * T::HP + T::HZ + VW * quad) * ES;  // row a centre in H
+    const uint32_t c_own = (2 * rp * T::TZ + VW * quad) * ES;               // row a in C/P/V tiles
 
     IsoCursor cu;
     cu.stage = 0; cu.phase = 0;
-    float4 qa[QL], qb[QL];
+    V qa[QL], qb[QL];
 #pragma unroll
-    for (int k = 0; k < QL; k++) { qa[k] = make_float4(0.f, 0.f, 0.f, 0.f); qb[k] = qa[k]; }
+    for (int k = 0; k < QL; k++) { const E zero[VW] = {}; arr_to_v(zero, qa[k]); qb[k] = qa[k]; }
 
-    bool sig_pending = P.sig_counter != nullptr;
+    bool sig_pending = FUSED && P.sig_counter != nullptr;
     for (cu.unit = blockIdx.x; cu.unit < nunits; cu.unit += gridDim.x) {
         if (sig_pending && cu.unit >= P.sig_units) { iso_boundary_arrive(P, lane); sig_pending = false; }   // (a CTA without boundary-first units)
         iso_unit_setup<T>(cu, P);
         const int ya = cu.y0 + 2 * rp;
-        const int zq = cu.z0 + 4 * quad;
-        const int nz_ok = max(0, min(4, P.z_end - zq));
+        const int zq = cu.z0 + VW * quad;
+        const int nz_ok = max(0, min(VW, P.z_end - zq));
         const int nva = (ya < P.y_end) ? nz_ok : 0;
         const int nvb = (ya + 1 < P.y_end) ? nz_ok : 0;
-        float* out_a = P.out + (long long)ya * P.out_sy + zq + (long long)cu.x0 * P.out_sx;       // plane x0; step s -> + dir*s planes
+        E* out_a = P.out + (long long)ya * P.out_sy + zq + (long long)cu.x0 * P.out_sx;       // plane x0; step s -> + dir*s planes
         const long long out_step = (long long)cu.dir * P.out_sx;
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(out_a) & 15) == 0);
         // this warp's boundary planes are complete after plane R-1 of its last boundary-first unit
@@ -301,11 +330,12 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
 #pragma unroll
                 for (int k = 0; k + U < QL; k++) { qa[k] = qa[k + U]; qb[k] = qb[k + U]; }
             }
-            qa[B + QN - 1] = *reinterpret_cast<const float4*>(st + T::C_OFF + c_own);
-            qb[B + QN - 1] = *reinterpret_cast<const float4*>(st + T::C_OFF + c_own + T::TZ * 4);
+            qa[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own);
+            qb[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own + T::TZ * ES);
 
-            if (MODE == 3) {
+            if constexpr (MODE == 3) {
                 // DEBUG (mem_probe=1): memory-system ceiling probe -- same TMA traffic and stores, no stencil math.
+                static_assert(sizeof(E) == 4, "the memory probe is compiled for fp32 only");
                 if (it >= 2 * R) {
                     const float4 pva = *reinterpret_cast<const float4*>(st + T::P_OFF + c_own);
                     const float4 vva = *reinterpret_cast<const float4*>(st + T::V_OFF + c_own);
@@ -319,66 +349,80 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
                     if (vec_ok && nvb == 4) stg128(oa + P.out_sy, rb);
                 }
             } else if (it >= 2 * R) {
-                const float* hp = reinterpret_cast<const float*>(st + T::H_OFF + h_own);
-                float pa[4], pb[4];
+                const E* hp = reinterpret_cast<const E*>(st + T::H_OFF + h_own);
+                E pa[VW], pb[VW];
                 f4_to_arr(qa[B + R], pa);
                 f4_to_arr(qb[B + R], pb);
                 // z windows of both rows (centre quads come from the queue)
-                float za[4 * (2 * ZQ + 1)], zb[4 * (2 * ZQ + 1)];
+                E za[VW * (2 * ZQ + 1)], zb[VW * (2 * ZQ + 1)];
 #pragma unroll
                 for (int k = -ZQ; k <= ZQ; k++) {
-                    if (k == 0) { f4_to_arr(qa[B + R], &za[4 * ZQ]); f4_to_arr(qb[B + R], &zb[4 * ZQ]); continue; }
-                    f4_to_arr(*reinterpret_cast<const float4*>(hp + 4 * k), &za[4 * (k + ZQ)]);
-                    f4_to_arr(*reinterpret_cast<const float4*>(hp + T::HP + 4 * k), &zb[4 * (k + ZQ)]);
+                    if (k == 0) { f4_to_arr(qa[B + R], &za[VW * ZQ]); f4_to_arr(qb[B + R], &zb[VW * ZQ]); continue; }
+                    f4_to_arr(*reinterpret_cast<const V*>(hp + VW * k), &za[VW * (k + ZQ)]);
+                    f4_to_arr(*reinterpret_cast<const V*>(hp + T::HP + VW * k), &zb[VW * (k + ZQ)]);
                 }
-                float acca[4] = {0.f, 0.f, 0.f, 0.f}, accb[4] = {0.f, 0.f, 0.f, 0.f};
+                E acca[VW] = {}, accb[VW] = {};
                 // y window: w(k) = hp + (k - R) * HP ; row a centre = w(R), row b centre = w(R+1)
-                float wlo_prev[4], whi_prev[4];   // w(R - (r-1)) and w(R+1 + (r-1)) from the previous radius
+                E wlo_prev[VW], whi_prev[VW];   // w(R - (r-1)) and w(R+1 + (r-1)) from the previous radius
                 f4_to_arr(qa[B + R], wlo_prev);   // r=1: row b's y-1 neighbour is row a's centre
                 f4_to_arr(qb[B + R], whi_prev);   //      row a's y+1 neighbour is row b's centre
 #pragma unroll
                 for (int r = 1; r <= R; r++) {
-                    float wlo[4], whi[4], xm[4], xp[4];
-                    f4_to_arr(*reinterpret_cast<const float4*>(hp - r * T::HP), wlo);        // row a - r
-                    f4_to_arr(*reinterpret_cast<const float4*>(hp + (r + 1) * T::HP), whi);  // row b + r
+                    E wlo[VW], whi[VW], xm[VW], xp[VW];
+                    f4_to_arr(*reinterpret_cast<const V*>(hp - r * T::HP), wlo);        // row a - r
+                    f4_to_arr(*reinterpret_cast<const V*>(hp + (r + 1) * T::HP), whi);  // row b + r
                     f4_to_arr(qa[B + R - r], xm); f4_to_arr(qa[B + R + r], xp);
 #pragma unroll
-                    for (int i = 0; i < 4; i++)   // row a: y-r = wlo, y+r = w(R+r) = previous whi
+                    for (int i = 0; i < VW; i++)   // row a: y-r = wlo, y+r = w(R+r) = previous whi
                         acca[i] = iso_group<MODE>(acca[i], pa[i], P.c[0], P.c[r], xm[i], xp[i], wlo[i], whi_prev[i],
-                                                  za[4 * ZQ + i - r], za[4 * ZQ + i + r], r == 1);
+                                                  za[VW * ZQ + i - r], za[VW * ZQ + i + r], r == 1);
                     f4_to_arr(qb[B + R - r], xm); f4_to_arr(qb[B + R + r], xp);
 #pragma unroll
-                    for (int i = 0; i < 4; i++)   // row b: y-r = w(R+1-r) = previous wlo, y+r = whi
+                    for (int i = 0; i < VW; i++)   // row b: y-r = w(R+1-r) = previous wlo, y+r = whi
                         accb[i] = iso_group<MODE>(accb[i], pb[i], P.c[0], P.c[r], xm[i], xp[i], wlo_prev[i], whi[i],
-                                                  zb[4 * ZQ + i - r], zb[4 * ZQ + i + r], r == 1);
+                                                  zb[VW * ZQ + i - r], zb[VW * ZQ + i + r], r == 1);
 #pragma unroll
-                    for (int i = 0; i < 4; i++) { wlo_prev[i] = wlo[i]; whi_prev[i] = whi[i]; }
+                    for (int i = 0; i < VW; i++) { wlo_prev[i] = wlo[i]; whi_prev[i] = whi[i]; }
                 }
-                const float4 pva = *reinterpret_cast<const float4*>(st + T::P_OFF + c_own);
-                const float4 vva = *reinterpret_cast<const float4*>(st + T::V_OFF + c_own);
-                const float4 pvb = *reinterpret_cast<const float4*>(st + T::P_OFF + c_own + T::TZ * 4);
-                const float4 vvb = *reinterpret_cast<const float4*>(st + T::V_OFF + c_own + T::TZ * 4);
-                float4 ra, rb;
-                ra.x = iso_final<MODE>(acca[0], pa[0], pva.x, vva.x); ra.y = iso_final<MODE>(acca[1], pa[1], pva.y, vva.y);
-                ra.z = iso_final<MODE>(acca[2], pa[2], pva.z, vva.z); ra.w = iso_final<MODE>(acca[3], pa[3], pva.w, vva.w);
-                rb.x = iso_final<MODE>(accb[0], pb[0], pvb.x, vvb.x); rb.y = iso_final<MODE>(accb[1], pb[1], pvb.y, vvb.y);
-                rb.z = iso_final<MODE>(accb[2], pb[2], pvb.z, vvb.z); rb.w = iso_final<MODE>(accb[3], pb[3], pvb.w, vvb.w);
-                float* oa = out_a + (long long)(it - 2 * R) * out_step;
-                float* ob = oa + P.out_sy;
-                if (vec_ok && nva == 4) { if (P.st_cs) stg128_cs(oa, ra); else stg128(oa, ra); }
-                else if (nva > 0) { oa[0] = ra.x; if (nva > 1) oa[1] = ra.y; if (nva > 2) oa[2] = ra.z; if (nva > 3) oa[3] = ra.w; }
-                if (vec_ok && nvb == 4) { if (P.st_cs) stg128_cs(ob, rb); else stg128(ob, rb); }
-                else if (nvb > 0) { ob[0] = rb.x; if (nvb > 1) ob[1] = rb.y; if (nvb > 2) ob[2] = rb.z; if (nvb > 3) ob[3] = rb.w; }
+                E pva[VW], vva[VW], pvb[VW], vvb[VW], ea[VW], eb[VW];
+                f4_to_arr(*reinterpret_cast<const V*>(st + T::P_OFF + c_own), pva);
+                f4_to_arr(*reinterpret_cast<const V*>(st + T::V_OFF + c_own), vva);
+                f4_to_arr(*reinterpret_cast<const V*>(st + T::P_OFF + c_own + T::TZ * ES), pvb);
+                f4_to_arr(*reinterpret_cast<const V*>(st + T::V_OFF + c_own + T::TZ * ES), vvb);
+#pragma unroll
+                for (int i = 0; i < VW; i++) ea[i] = iso_final<MODE>(acca[i], pa[i], pva[i], vva[i]);
+#pragma unroll
+                for (int i = 0; i < VW; i++) eb[i] = iso_final<MODE>(accb[i], pb[i], pvb[i], vvb[i]);
+                V ra, rb;
+                arr_to_v(ea, ra); arr_to_v(eb, rb);
+                E* oa = out_a + (long long)(it - 2 * R) * out_step;
+                E* ob = oa + P.out_sy;
+                if (vec_ok && nva == VW) { if (P.st_cs) stg128_cs(oa, ra); else stg128(oa, ra); }
+                else {
+#pragma unroll
+                    for (int i = 0; i < VW && i < nva; i++) oa[i] = ea[i];
+                }
+                if (vec_ok && nvb == VW) { if (P.st_cs) stg128_cs(ob, rb); else stg128(ob, rb); }
+                else {
+#pragma unroll
+                    for (int i = 0; i < VW && i < nvb; i++) ob[i] = eb[i];
+                }
                 // fused halo exchange: boundary planes also go straight into the x neighbours' halo cells
                 const int xo = cu.x0 + cu.dir * (it - 2 * R);
-                float* peer = (P.peer_lo != nullptr && xo < R) ? P.peer_lo : ((P.peer_hi != nullptr && xo >= P.nx - R) ? P.peer_hi : nullptr);
+                E* peer = !FUSED ? nullptr : (P.peer_lo != nullptr && xo < R) ? P.peer_lo : ((P.peer_hi != nullptr && xo >= P.nx - R) ? P.peer_hi : nullptr);
                 if (peer != nullptr && P.peer_probe != 1) {
-                    float* qa_ = peer + (oa - P.out);
-                    float* qb_ = qa_ + P.out_sy;
-                    if (vec_ok && nva == 4) stg128(qa_, ra);
-                    else if (nva > 0) { qa_[0] = ra.x; if (nva > 1) qa_[1] = ra.y; if (nva > 2) qa_[2] = ra.z; if (nva > 3) qa_[3] = ra.w; }
-                    if (vec_ok && nvb == 4) stg128(qb_, rb);
-                    else if (nvb > 0) { qb_[0] = rb.x; if (nvb > 1) qb_[1] = rb.y; if (nvb > 2) qb_[2] = rb.z; if (nvb > 3) qb_[3] = rb.w; }
+                    E* qa_ = peer + (oa - P.out);
+                    E* qb_ = qa_ + P.out_sy;
+                    if (vec_ok && nva == VW) stg128(qa_, ra);
+                    else {
+#pragma unroll
+                        for (int i = 0; i < VW && i < nva; i++) qa_[i] = ea[i];
+                    }
+                    if (vec_ok && nvb == VW) stg128(qb_, rb);
+                    else {
+#pragma unroll
+                        for (int i = 0; i < VW && i < nvb; i++) qb_[i] = eb[i];
+                    }
                 }
             }
             __syncwarp();

@@ -125,4 +125,12 @@ __device__ __forceinline__ void stg128_cs(float* p, float4 v) {
     asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
+__device__ __forceinline__ void stg128(double* p, double2 v) {
+    asm volatile("st.global.v2.f64 [%0], {%1, %2};" ::"l"(p), "d"(v.x), "d"(v.y) : "memory");
+}
+
+__device__ __forceinline__ void stg128_cs(double* p, double2 v) {
+    asm volatile("st.global.cs.v2.f64 [%0], {%1, %2};" ::"l"(p), "d"(v.x), "d"(v.y) : "memory");
+}
+
 }  // namespace yb
