@@ -504,12 +504,18 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     int64_t w[3] = {0, 0, 0};
     for (int d = 0; d < s.ndd && split; d++) {
         if (s.num_ranks[d] <= 1) continue;
+        // In a unit-stride dim every box starts on a 16-byte boundary (the rank's domain origin is 128-B aligned): the TMA
+        // sweep kernels need that, and a box start off it faults on an H100.  So the exterior slabs there are w rounded up
+        // to whole 16-byte vectors wide -- up to 3 (fp32) or 1 (fp64) planes more -- and the interior keeps its sweep.
+        int64_t al = 1;
         for (auto& v : s.vars) {
             const Dim* dd = v.domain_dim(d);
-            if (dd) w[d] = std::max<int64_t>(w[d], std::max(dd->spec.halo_l, dd->spec.halo_r));
+            if (!dd) continue;
+            w[d] = std::max<int64_t>(w[d], std::max(dd->spec.halo_l, dd->spec.halo_r));
+            if (dd->stride == 1) al = std::max<int64_t>(al, 16 / v.elem_bytes);
         }
-        if (s.rank_index[d] > 0) interior.b[d] += w[d];
-        if (s.rank_index[d] < s.num_ranks[d] - 1) interior.e[d] -= w[d];
+        if (s.rank_index[d] > 0) interior.b[d] += (w[d] + al - 1) / al * al;
+        if (s.rank_index[d] < s.num_ranks[d] - 1) interior.e[d] = std::max<int64_t>(0, interior.e[d] - w[d]) / al * al;
         if (interior.e[d] - interior.b[d] < 1) split = false;
     }
     if (!split) {

@@ -443,6 +443,11 @@ struct IsoEngine : Engine {
             if (box.e[1] - box.b[1] < 8 || box.e[2] - box.b[2] < 16) use_tma = false;
         }
         if (kernel == "tma" && !maps_ok) return set_error(YB_EUNSUPPORTED, "the tiled TMA kernel needs sm_90+");
+        // TMA box loads whose z start is off a 16-byte boundary fault on an H100 (halo_run_stage never asks for such a box)
+        if (use_tma && (box.b[2] * int64_t(sizeof(E))) % 16 != 0) {
+            if (kernel == "tma") return set_error(YB_EUNSUPPORTED, "the tiled TMA kernel needs boxes that start on a 16-byte boundary in z");
+            use_tma = false;
+        }
         if (use_tma) {
             const int ti = radius == 8 ? tile : 0;      // other radii and fp64: one compiled variant
             const TileCfgT<E>& c = sweep_cfg<E>();
