@@ -200,6 +200,20 @@ const TileCfg& tile_cfg(int i) {
     return cfgs[i];
 }
 
+// Resident-plane form (option `resident`, iso3dfd_tma3_kernel) of the radius-8 producer-warpgroup, 2-planes-per-trip variants:
+// same tile shapes, so it shares their tensor maps.  Rings within the 227 KB opt-in: 16x128 (18 KB slots) 10 slots = 1 plane of
+// prefetch; 32x64 (15 KB slots) 12 slots = 3 planes; both with 2 stages of p(t-1) / v.  nullptr for the other tiles.
+template <class T>
+TileCfg cfg_resident(const char* name) {
+    return TileCfg{true, name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128, T::SMEM_BYTES,
+                   {iso3dfd_tma3_kernel<T, 0>, iso3dfd_tma3_kernel<T, 1>, iso3dfd_tma3_kernel<T, 2>, iso3dfd_tma3_kernel<T, 3>}};
+}
+const TileCfg* resident_cfg(int tile) {
+    static const TileCfg cfgs[2] = {cfg_resident<IsoTile3<8, 16, 16, 12, 2>>("32x64 resident planes, 12 slots"),
+                                    cfg_resident<IsoTile3<8, 8, 32, 10, 2>>("16x128 resident planes, 10 slots")};
+    return tile == 6 ? &cfgs[0] : tile == 7 ? &cfgs[1] : nullptr;
+}
+
 // ---- temporal tile (yb_iso3dfd_tt.cuh): compiled variants per radius and FP mode ----
 typedef void (*TTKernelFn)(const TTMaps, const TTParams);
 struct TTCfg {
@@ -249,10 +263,11 @@ struct IsoEngine : Engine {
     double coef[ISO_MAX_R + 1] = {0};
     std::string kernel = "auto";   // auto | tma | direct
     int tile = DEFAULT_TILE;       // index into tile_cfg(): 16x128, producer warpgroup, 2 planes per trip
+    bool resident = true;          // tiles 6 and 7 at radius 8 in fp32: their resident-plane form (resident_cfg())
     int lx = 0;                    // planes per sweep chunk (0 = choose per launch)
     int grid_override = 0;
     int num_sms = 148;
-    bool attr_set[NTILES][4] = {};
+    bool attr_set[NTILES + 2][4] = {};    // [cfg_index()][FP mode]
     // L2 policy of the sweep: both p(t) streams evict_last (a plane is fetched halo-less 8 sweep steps before it is fetched
     // with its halo, and its halo rows are the neighbouring tiles' centre rows), p(t-1) / v evict_first (streamed once), results
     // leave with streaming stores
@@ -282,6 +297,7 @@ struct IsoEngine : Engine {
             if (t < 0 || t >= NTILES) return YB_EINVAL;
             tile = t;
         }
+        else if (k == "resident") { resident = atoi(v.c_str()) != 0; }
         else if (k == "lx") { lx = std::max(0, atoi(v.c_str())); }
         else if (k == "grid") { grid_override = std::max(0, atoi(v.c_str())); }
         else if (k == "mem_probe") { mem_probe = atoi(v.c_str()) != 0; }
@@ -315,9 +331,10 @@ struct IsoEngine : Engine {
         else return YB_EINVAL;
         return 0;
     }
-    bool get_option(const Solution&, const std::string& k, std::string& v) const override {
+    bool get_option(const Solution& s, const std::string& k, std::string& v) const override {
         if (k == "kernel") v = kernel;
         else if (k == "tile") v = std::to_string(tile);
+        else if (k == "resident") v = (s.spec.radius == 8 && s.spec.elem_bytes == 4 && resident && resident_cfg(tile)) ? "1" : "0";
         else if (k == "lx") v = std::to_string(lx);
         else if (k == "grid") v = std::to_string(grid_override);
         else if (k == "block_steps") v = std::to_string(block_steps);
@@ -368,7 +385,7 @@ struct IsoEngine : Engine {
                     for (int m = 0; m < 3; m++) preload_kernel((const void*)tt_radius_cfg(radius, vr)->fn[m]);
                 preload_kernel((const void*)slot_box_copy_kernel);
             }
-            const TileCfg& c = radius == 8 ? tile_cfg(tile) : *iso_radius_cfg(radius);
+            const TileCfg& c = sweep_cfg<float>();
             for (int m = 0; m < 4; m++) preload_kernel((const void*)c.fn[m]);
         }
         if (f64) {
@@ -394,12 +411,16 @@ struct IsoEngine : Engine {
         return make_map(&m.v, v, 0, c.tz, c.ty);
     }
 
-    // The sweep variant a launch uses: the selected tile at radius 8, the one compiled variant at other radii.
+    // The sweep variant a launch uses: the selected tile (in its resident-plane form where it has one and `resident` is on) at
+    // radius 8, the one compiled variant at other radii.
+    bool resident_on() const { return radius == 8 && !f64 && resident && resident_cfg(tile); }
     template <class E>
     const TileCfgT<E>& sweep_cfg() const {
         if constexpr (sizeof(E) == 8) return *iso_radius_cfg_f64(radius);
-        else return radius == 8 ? tile_cfg(tile) : *iso_radius_cfg(radius);
+        else return radius != 8 ? *iso_radius_cfg(radius) : resident_on() ? *resident_cfg(tile) : tile_cfg(tile);
     }
+    // Row of attr_set: the tile at radius 8 (NTILES + 0 / 1: resident forms of tiles 6 / 7), 0 otherwise.
+    int cfg_index() const { return radius != 8 ? 0 : resident_on() ? NTILES + (tile == 7) : tile; }
 
     template <class E>
     void fill_params(const Solution& s, int64_t t, const Box& box, IsoParamsT<E>& P) const {
@@ -449,7 +470,8 @@ struct IsoEngine : Engine {
             use_tma = false;
         }
         if (use_tma) {
-            const int ti = radius == 8 ? tile : 0;      // other radii and fp64: one compiled variant
+            const int ti = radius == 8 ? tile : 0;      // tensor maps; other radii and fp64: one compiled variant
+            const int ai = cfg_index();
             const TileCfgT<E>& c = sweep_cfg<E>();
             if (mem_probe && c.fn[3]) mode = 3;
             // fused halo exchange: only for whole-domain launches of a kernel that implements the peer stores
@@ -519,9 +541,9 @@ struct IsoEngine : Engine {
                 P.sig_epoch = s.fused_x.epoch;
                 s.fused_x.signalled = true;
             }
-            if (!attr_set[ti][mode]) {
+            if (!attr_set[ai][mode]) {
                 YB_CUDA(cudaFuncSetAttribute(c.fn[mode], cudaFuncAttributeMaxDynamicSharedMemorySize, int(c.smem)));
-                attr_set[ti][mode] = true;
+                attr_set[ai][mode] = true;
             }
             c.fn[mode]<<<grid, c.threads, c.smem, st>>>(maps[ti][cur], P);
         } else {
@@ -641,7 +663,7 @@ struct IsoEngine : Engine {
         tile = TUNE_TILES[v / 3]; lx = TUNE_LXS[v % 3];
         s.options["tile"] = std::to_string(tile);
         s.options["lx"] = std::to_string(lx);
-        preload_kernel((const void*)tile_cfg(tile).fn[s.fp_mode]);
+        preload_kernel((const void*)sweep_cfg<float>().fn[s.fp_mode]);
     }
     std::string tune_describe(const Solution&, int v) const override {
         char b[160];
@@ -684,8 +706,8 @@ struct IsoEngine : Engine {
         return 0;
     }
 
-    // Offline tuner: the compiled sweep variants (tile shape, producer warpgroup, planes per trip) x sweep chunk
-    // lengths, timed over the whole rank box; the analogue of the reference's block-size search
+    // Offline tuner: the compiled sweep variants (tile shape, producer warpgroup, planes per trip, resident planes) x sweep
+    // chunk lengths, timed over the whole rank box; the analogue of the reference's block-size search
     // (/root/reference/src/kernel/lib/auto_tuner.cpp) for the knobs this engine has.  fp64 has one variant per radius: only
     // the chunk length is searched.
     int auto_tune(Solution& s, cudaStream_t st, std::string& report) override {
@@ -695,28 +717,34 @@ struct IsoEngine : Engine {
         for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = s.rank_size[d]; }
         if (whole.e[1] < 8 || whole.e[2] < 16) { report = "iso3dfd: domain too thin for the tiled kernel"; return 0; }
         const int64_t t0 = s.vars[0].last_valid_step();
-        const std::vector<int> tiles = f64 ? std::vector<int>{tile} : std::vector<int>{7, 6, 5, 4, 1, 0};
+        // (tile, resident) pairs; resident = 1 only where the tile has a resident-plane form
+        const std::vector<std::pair<int, bool>> forms =
+            f64 ? std::vector<std::pair<int, bool>>{{tile, false}}
+                : std::vector<std::pair<int, bool>>{{7, true}, {6, true}, {7, false}, {6, false}, {5, false}, {4, false}, {1, false}, {0, false}};
         const int lxs[] = {0, 256, 512, 1024};   // planes per interior chunk (0 = cost model)
         const int keep_tile = tile, keep_lx = lx;
+        const bool keep_res = resident;
         double best = 1e30;
         int best_tile = tile, best_lx = lx;
+        bool best_res = resident;
         char line[160];
         report.clear();
-        for (int ti : tiles)
+        for (const auto& [ti, res] : forms)
             for (int l : lxs) {
                 if (l > whole.e[0]) continue;
-                tile = ti; lx = l;
+                tile = ti; resident = res; lx = l;
                 int64_t t = t0;
                 const double ms = time_launches(st, 3, [&]() { return launch(s, 0, t++, whole, st); });
-                if (ms < 0) { tile = keep_tile; lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-                snprintf(line, sizeof line, " tile=%d (%s) lx=%d: %.4f ms/step\n", ti, f64 ? iso_radius_cfg_f64(radius)->name : tile_cfg(ti).name, l, ms);
+                if (ms < 0) { tile = keep_tile; resident = keep_res; lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
+                snprintf(line, sizeof line, " tile=%d resident=%d (%s) lx=%d: %.4f ms/step\n", ti, int(resident_on()), f64 ? iso_radius_cfg_f64(radius)->name : sweep_cfg<float>().name, l, ms);
                 report += line;
-                if (ms < best) { best = ms; best_tile = ti; best_lx = l; }
+                if (ms < best) { best = ms; best_tile = ti; best_res = res; best_lx = l; }
             }
-        tile = best_tile; lx = best_lx;
-        snprintf(line, sizeof line, "best: tile=%d lx=%d (%.4f ms/step)\n", tile, lx, best);
+        tile = best_tile; resident = best_res; lx = best_lx;
+        snprintf(line, sizeof line, "best: tile=%d resident=%d lx=%d (%.4f ms/step)\n", tile, int(resident_on()), lx, best);
         report += line;
         s.options["tile"] = std::to_string(tile);
+        s.options["resident"] = resident ? "1" : "0";
         s.options["lx"] = std::to_string(lx);
         return 0;
     }

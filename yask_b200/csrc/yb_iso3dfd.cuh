@@ -217,6 +217,112 @@ __device__ __forceinline__ void f4_to_arr(const double2& v, double* a) { a[0] = 
 __device__ __forceinline__ void arr_to_v(const float* a, float4& v) { v = make_float4(a[0], a[1], a[2], a[3]); }
 __device__ __forceinline__ void arr_to_v(const double* a, double2& v) { v = make_double2(a[0], a[1]); }
 
+// One sweep step of a consumer thread: p(t+1) of its two rows (a, b) at plane xo, and the stores.  Shared by the sweep kernels
+// (iso3dfd_tma2_kernel, iso3dfd_tma3_kernel), which differ only in how p(t) reaches shared memory.
+//   qa, qb  the rows' x queues; window q[B .. B+2R], centre q[B+R]
+//   h       row a's centre in the haloed p(t) plane (T::HP elements per row; row b is the next row)
+//   pv, v   row a in the p(t-1) and v tiles (T::TZ elements per row)
+//   oa      row a's output vector; row b is P.out_sy further on
+// Results leave as 128-bit stores where the row's vector is whole and aligned (scalars on ragged edges).  The fused halo
+// exchange (peer stores into the x neighbours' halo cells) is compiled for fp32 only: the fp64 sweep is listed with
+// fused_ok = false, and leaving the out-of-line signal call out keeps its registers free of call spills.
+template <class T, int MODE, int B, int QL>
+__device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>& P, const typename T::V (&qa)[QL],
+                                                const typename T::V (&qb)[QL], const uint8_t* h, const uint8_t* pv,
+                                                const uint8_t* v, typename T::E* oa, int xo, int nva, int nvb, bool vec_ok) {
+    using E = typename T::E;
+    using V = typename T::V;
+    constexpr int R = T::R, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
+    constexpr bool FUSED = sizeof(E) == 4;
+    if constexpr (MODE == 3) {
+        // DEBUG (mem_probe=1): memory-system ceiling probe -- same TMA traffic and stores, no stencil math.
+        static_assert(sizeof(E) == 4, "the memory probe is compiled for fp32 only");
+        const float4 pva = *reinterpret_cast<const float4*>(pv);
+        const float4 vva = *reinterpret_cast<const float4*>(v);
+        const float4 pvb = *reinterpret_cast<const float4*>(pv + T::TZ * 4);
+        const float4 vvb = *reinterpret_cast<const float4*>(v + T::TZ * 4);
+        const float4 ha = *reinterpret_cast<const float4*>(h);
+        float4 ra = make_float4(pva.x + vva.x * qa[B + R].x, pva.y + vva.y * ha.y, pva.z + vva.z, pva.w + vva.w);
+        float4 rb = make_float4(pvb.x + vvb.x * qb[B + R].x, pvb.y + vvb.y, pvb.z + vvb.z, pvb.w + vvb.w);
+        if (vec_ok && nva == 4) stg128(oa, ra);
+        if (vec_ok && nvb == 4) stg128(oa + P.out_sy, rb);
+    } else {
+        const E* hp = reinterpret_cast<const E*>(h);
+        E pa[VW], pb[VW];
+        f4_to_arr(qa[B + R], pa);
+        f4_to_arr(qb[B + R], pb);
+        // z windows of both rows (centre quads come from the queue)
+        E za[VW * (2 * ZQ + 1)], zb[VW * (2 * ZQ + 1)];
+#pragma unroll
+        for (int k = -ZQ; k <= ZQ; k++) {
+            if (k == 0) { f4_to_arr(qa[B + R], &za[VW * ZQ]); f4_to_arr(qb[B + R], &zb[VW * ZQ]); continue; }
+            f4_to_arr(*reinterpret_cast<const V*>(hp + VW * k), &za[VW * (k + ZQ)]);
+            f4_to_arr(*reinterpret_cast<const V*>(hp + T::HP + VW * k), &zb[VW * (k + ZQ)]);
+        }
+        E acca[VW] = {}, accb[VW] = {};
+        // y window: w(k) = hp + (k - R) * HP ; row a centre = w(R), row b centre = w(R+1)
+        E wlo_prev[VW], whi_prev[VW];   // w(R - (r-1)) and w(R+1 + (r-1)) from the previous radius
+        f4_to_arr(qa[B + R], wlo_prev);   // r=1: row b's y-1 neighbour is row a's centre
+        f4_to_arr(qb[B + R], whi_prev);   //      row a's y+1 neighbour is row b's centre
+#pragma unroll
+        for (int r = 1; r <= R; r++) {
+            E wlo[VW], whi[VW], xm[VW], xp[VW];
+            f4_to_arr(*reinterpret_cast<const V*>(hp - r * T::HP), wlo);        // row a - r
+            f4_to_arr(*reinterpret_cast<const V*>(hp + (r + 1) * T::HP), whi);  // row b + r
+            f4_to_arr(qa[B + R - r], xm); f4_to_arr(qa[B + R + r], xp);
+#pragma unroll
+            for (int i = 0; i < VW; i++)   // row a: y-r = wlo, y+r = w(R+r) = previous whi
+                acca[i] = iso_group<MODE>(acca[i], pa[i], P.c[0], P.c[r], xm[i], xp[i], wlo[i], whi_prev[i],
+                                          za[VW * ZQ + i - r], za[VW * ZQ + i + r], r == 1);
+            f4_to_arr(qb[B + R - r], xm); f4_to_arr(qb[B + R + r], xp);
+#pragma unroll
+            for (int i = 0; i < VW; i++)   // row b: y-r = w(R+1-r) = previous wlo, y+r = whi
+                accb[i] = iso_group<MODE>(accb[i], pb[i], P.c[0], P.c[r], xm[i], xp[i], wlo_prev[i], whi[i],
+                                          zb[VW * ZQ + i - r], zb[VW * ZQ + i + r], r == 1);
+#pragma unroll
+            for (int i = 0; i < VW; i++) { wlo_prev[i] = wlo[i]; whi_prev[i] = whi[i]; }
+        }
+        E pva[VW], vva[VW], pvb[VW], vvb[VW], ea[VW], eb[VW];
+        f4_to_arr(*reinterpret_cast<const V*>(pv), pva);
+        f4_to_arr(*reinterpret_cast<const V*>(v), vva);
+        f4_to_arr(*reinterpret_cast<const V*>(pv + T::TZ * ES), pvb);
+        f4_to_arr(*reinterpret_cast<const V*>(v + T::TZ * ES), vvb);
+#pragma unroll
+        for (int i = 0; i < VW; i++) ea[i] = iso_final<MODE>(acca[i], pa[i], pva[i], vva[i]);
+#pragma unroll
+        for (int i = 0; i < VW; i++) eb[i] = iso_final<MODE>(accb[i], pb[i], pvb[i], vvb[i]);
+        V ra, rb;
+        arr_to_v(ea, ra); arr_to_v(eb, rb);
+        E* ob = oa + P.out_sy;
+        if (vec_ok && nva == VW) { if (P.st_cs) stg128_cs(oa, ra); else stg128(oa, ra); }
+        else {
+#pragma unroll
+            for (int i = 0; i < VW && i < nva; i++) oa[i] = ea[i];
+        }
+        if (vec_ok && nvb == VW) { if (P.st_cs) stg128_cs(ob, rb); else stg128(ob, rb); }
+        else {
+#pragma unroll
+            for (int i = 0; i < VW && i < nvb; i++) ob[i] = eb[i];
+        }
+        // fused halo exchange: boundary planes also go straight into the x neighbours' halo cells
+        E* peer = !FUSED ? nullptr : (P.peer_lo != nullptr && xo < R) ? P.peer_lo : ((P.peer_hi != nullptr && xo >= P.nx - R) ? P.peer_hi : nullptr);
+        if (peer != nullptr && P.peer_probe != 1) {
+            E* qa_ = peer + (oa - P.out);
+            E* qb_ = qa_ + P.out_sy;
+            if (vec_ok && nva == VW) stg128(qa_, ra);
+            else {
+#pragma unroll
+                for (int i = 0; i < VW && i < nva; i++) qa_[i] = ea[i];
+            }
+            if (vec_ok && nvb == VW) stg128(qb_, rb);
+            else {
+#pragma unroll
+                for (int i = 0; i < VW && i < nvb; i++) qb_[i] = eb[i];
+            }
+        }
+    }
+}
+
 // PW = 1: a dedicated producer warp (warp NWARPS) issues the TMA loads, so no compute warp carries the
 //         issue code (with 2 warps per scheduler a straggling warp 0 delays every stage hand-over).
 // U  = 2: the sweep loop handles two planes per trip and rotates the x queues by two entries every second
@@ -228,9 +334,7 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
     using V = typename T::V;
     constexpr int R = T::R, QN = T::QN, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
     constexpr int QL = QN + (U - 1);          // queue entries kept per row
-    // The fused halo exchange (peer stores + completion signal) is compiled for fp32 only: the fp64 sweep is listed with
-    // fused_ok = false, and leaving the out-of-line signal call out keeps its registers free of call spills.
-    constexpr bool FUSED = sizeof(E) == 4;
+    constexpr bool FUSED = sizeof(E) == 4;    // see iso_rows_update
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     uint8_t* sbase = smem_raw + (base - smem_u32(smem_raw));
@@ -333,98 +437,9 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
             qa[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own);
             qb[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own + T::TZ * ES);
 
-            if constexpr (MODE == 3) {
-                // DEBUG (mem_probe=1): memory-system ceiling probe -- same TMA traffic and stores, no stencil math.
-                static_assert(sizeof(E) == 4, "the memory probe is compiled for fp32 only");
-                if (it >= 2 * R) {
-                    const float4 pva = *reinterpret_cast<const float4*>(st + T::P_OFF + c_own);
-                    const float4 vva = *reinterpret_cast<const float4*>(st + T::V_OFF + c_own);
-                    const float4 pvb = *reinterpret_cast<const float4*>(st + T::P_OFF + c_own + T::TZ * 4);
-                    const float4 vvb = *reinterpret_cast<const float4*>(st + T::V_OFF + c_own + T::TZ * 4);
-                    const float4 ha = *reinterpret_cast<const float4*>(st + T::H_OFF + h_own);
-                    float4 ra = make_float4(pva.x + vva.x * qa[B + R].x, pva.y + vva.y * ha.y, pva.z + vva.z, pva.w + vva.w);
-                    float4 rb = make_float4(pvb.x + vvb.x * qb[B + R].x, pvb.y + vvb.y, pvb.z + vvb.z, pvb.w + vvb.w);
-                    float* oa = out_a + (long long)(it - 2 * R) * out_step;
-                    if (vec_ok && nva == 4) stg128(oa, ra);
-                    if (vec_ok && nvb == 4) stg128(oa + P.out_sy, rb);
-                }
-            } else if (it >= 2 * R) {
-                const E* hp = reinterpret_cast<const E*>(st + T::H_OFF + h_own);
-                E pa[VW], pb[VW];
-                f4_to_arr(qa[B + R], pa);
-                f4_to_arr(qb[B + R], pb);
-                // z windows of both rows (centre quads come from the queue)
-                E za[VW * (2 * ZQ + 1)], zb[VW * (2 * ZQ + 1)];
-#pragma unroll
-                for (int k = -ZQ; k <= ZQ; k++) {
-                    if (k == 0) { f4_to_arr(qa[B + R], &za[VW * ZQ]); f4_to_arr(qb[B + R], &zb[VW * ZQ]); continue; }
-                    f4_to_arr(*reinterpret_cast<const V*>(hp + VW * k), &za[VW * (k + ZQ)]);
-                    f4_to_arr(*reinterpret_cast<const V*>(hp + T::HP + VW * k), &zb[VW * (k + ZQ)]);
-                }
-                E acca[VW] = {}, accb[VW] = {};
-                // y window: w(k) = hp + (k - R) * HP ; row a centre = w(R), row b centre = w(R+1)
-                E wlo_prev[VW], whi_prev[VW];   // w(R - (r-1)) and w(R+1 + (r-1)) from the previous radius
-                f4_to_arr(qa[B + R], wlo_prev);   // r=1: row b's y-1 neighbour is row a's centre
-                f4_to_arr(qb[B + R], whi_prev);   //      row a's y+1 neighbour is row b's centre
-#pragma unroll
-                for (int r = 1; r <= R; r++) {
-                    E wlo[VW], whi[VW], xm[VW], xp[VW];
-                    f4_to_arr(*reinterpret_cast<const V*>(hp - r * T::HP), wlo);        // row a - r
-                    f4_to_arr(*reinterpret_cast<const V*>(hp + (r + 1) * T::HP), whi);  // row b + r
-                    f4_to_arr(qa[B + R - r], xm); f4_to_arr(qa[B + R + r], xp);
-#pragma unroll
-                    for (int i = 0; i < VW; i++)   // row a: y-r = wlo, y+r = w(R+r) = previous whi
-                        acca[i] = iso_group<MODE>(acca[i], pa[i], P.c[0], P.c[r], xm[i], xp[i], wlo[i], whi_prev[i],
-                                                  za[VW * ZQ + i - r], za[VW * ZQ + i + r], r == 1);
-                    f4_to_arr(qb[B + R - r], xm); f4_to_arr(qb[B + R + r], xp);
-#pragma unroll
-                    for (int i = 0; i < VW; i++)   // row b: y-r = w(R+1-r) = previous wlo, y+r = whi
-                        accb[i] = iso_group<MODE>(accb[i], pb[i], P.c[0], P.c[r], xm[i], xp[i], wlo_prev[i], whi[i],
-                                                  zb[VW * ZQ + i - r], zb[VW * ZQ + i + r], r == 1);
-#pragma unroll
-                    for (int i = 0; i < VW; i++) { wlo_prev[i] = wlo[i]; whi_prev[i] = whi[i]; }
-                }
-                E pva[VW], vva[VW], pvb[VW], vvb[VW], ea[VW], eb[VW];
-                f4_to_arr(*reinterpret_cast<const V*>(st + T::P_OFF + c_own), pva);
-                f4_to_arr(*reinterpret_cast<const V*>(st + T::V_OFF + c_own), vva);
-                f4_to_arr(*reinterpret_cast<const V*>(st + T::P_OFF + c_own + T::TZ * ES), pvb);
-                f4_to_arr(*reinterpret_cast<const V*>(st + T::V_OFF + c_own + T::TZ * ES), vvb);
-#pragma unroll
-                for (int i = 0; i < VW; i++) ea[i] = iso_final<MODE>(acca[i], pa[i], pva[i], vva[i]);
-#pragma unroll
-                for (int i = 0; i < VW; i++) eb[i] = iso_final<MODE>(accb[i], pb[i], pvb[i], vvb[i]);
-                V ra, rb;
-                arr_to_v(ea, ra); arr_to_v(eb, rb);
-                E* oa = out_a + (long long)(it - 2 * R) * out_step;
-                E* ob = oa + P.out_sy;
-                if (vec_ok && nva == VW) { if (P.st_cs) stg128_cs(oa, ra); else stg128(oa, ra); }
-                else {
-#pragma unroll
-                    for (int i = 0; i < VW && i < nva; i++) oa[i] = ea[i];
-                }
-                if (vec_ok && nvb == VW) { if (P.st_cs) stg128_cs(ob, rb); else stg128(ob, rb); }
-                else {
-#pragma unroll
-                    for (int i = 0; i < VW && i < nvb; i++) ob[i] = eb[i];
-                }
-                // fused halo exchange: boundary planes also go straight into the x neighbours' halo cells
-                const int xo = cu.x0 + cu.dir * (it - 2 * R);
-                E* peer = !FUSED ? nullptr : (P.peer_lo != nullptr && xo < R) ? P.peer_lo : ((P.peer_hi != nullptr && xo >= P.nx - R) ? P.peer_hi : nullptr);
-                if (peer != nullptr && P.peer_probe != 1) {
-                    E* qa_ = peer + (oa - P.out);
-                    E* qb_ = qa_ + P.out_sy;
-                    if (vec_ok && nva == VW) stg128(qa_, ra);
-                    else {
-#pragma unroll
-                        for (int i = 0; i < VW && i < nva; i++) qa_[i] = ea[i];
-                    }
-                    if (vec_ok && nvb == VW) stg128(qb_, rb);
-                    else {
-#pragma unroll
-                        for (int i = 0; i < VW && i < nvb; i++) qb_[i] = eb[i];
-                    }
-                }
-            }
+            if (it >= 2 * R)
+                iso_rows_update<T, MODE, B>(P, qa, qb, st + T::H_OFF + h_own, st + T::P_OFF + c_own, st + T::V_OFF + c_own,
+                                            out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb, vec_ok);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[cu.stage]);
             if (++cu.stage == T::STAGES) { cu.stage = 0; cu.phase ^= 1u; }
@@ -441,6 +456,163 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
                 step(std::integral_constant<int, 0>{}, it);
                 if (it + 1 < cu.n_it) step(std::integral_constant<int, U - 1>{}, it + 1);
             }
+        }
+    }
+    if (sig_pending) iso_boundary_arrive(P, lane);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Resident-plane sweep (fp32): every p(t) plane is loaded ONCE, with its halo, into a ring of NS shared-memory slots.
+//
+// The sweep kernel above loads each plane twice: halo-less R steps ahead to feed the x queues, and again with its halo when it
+// becomes the current plane.  Between the two fetches a CTA streams ~R planes of traffic, and the whole grid together about as
+// much as the H100's L2 holds, so the second fetch goes back to HBM.  Here the slot that receives plane x+R feeds the queues
+// from its centre rows and stays resident until plane x is computed, R steps later, from its halo rows; only then do the
+// consumer warps release it.  Queue-only planes (the R planes before a chunk and the R after it) take the halo-less box and are
+// released at once.  p(t-1) and v arrive in a ring of their own, NPV stages.  NS = R + 1 + (planes of prefetch).
+// Thread layout, x queues (two planes per trip), producer warpgroup and arithmetic are those of iso3dfd_tma2_kernel<T,MODE,1,2>.
+// ---------------------------------------------------------------------------------------------
+template <int R_, int TYP_, int TZQ_, int NS_, int NPV_>
+struct IsoTile3 : IsoTile2<R_, TYP_, TZQ_, 1, float> {
+    using Base = IsoTile2<R_, TYP_, TZQ_, 1, float>;
+    static constexpr int NS = NS_, NPV = NPV_;
+    static_assert(NS > R_ + 1, "a slot lives R + 1 sweep steps; at least one more is prefetch");
+    static constexpr uint32_t SLOT_BYTES = (Base::H_BYTES + 127) / 128 * 128;
+    static constexpr uint32_t PV_OFF = NS * SLOT_BYTES;
+    static constexpr uint32_t PV_BYTES = 2 * Base::C_BYTES;     // p(t-1) tile, then v tile
+    static constexpr uint32_t BAR_OFF = PV_OFF + NPV * PV_BYTES;
+    static constexpr uint32_t SMEM_BYTES = BAR_OFF + 2 * (NS + NPV) * 8 + 128;
+    static_assert(SMEM_BYTES <= 232448, "over the sm_90 opt-in shared memory per block");
+};
+
+template <class T, int MODE>
+__global__ void __launch_bounds__(T::THREADS + 128, 1)
+iso3dfd_tma3_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ IsoParams P) {
+    using V = float4;
+    constexpr int R = T::R, QN = T::QN, NS = T::NS, NPV = T::NPV, ES = 4;
+    constexpr int QL = QN + 1;                // two planes per trip: one extra queue entry per row
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
+    uint8_t* sbase = smem_raw + (base - smem_u32(smem_raw));
+    uint64_t* h_full = reinterpret_cast<uint64_t*>(sbase + T::BAR_OFF);
+    uint64_t* h_empty = h_full + NS;
+    uint64_t* pv_full = h_empty + NS;
+    uint64_t* pv_empty = pv_full + NPV;
+
+    const int tid = threadIdx.x;
+    const int lane = tid & 31;
+    const int nunits = P.nty * P.ntz * P.nchunks;
+
+    if (tid == 0) {
+        tma_prefetch_desc(&M.h); tma_prefetch_desc(&M.c); tma_prefetch_desc(&M.p); tma_prefetch_desc(&M.v);
+        for (int s = 0; s < NS; s++) { mbar_init(&h_full[s], 1); mbar_init(&h_empty[s], T::NWARPS); }
+        for (int s = 0; s < NPV; s++) { mbar_init(&pv_full[s], 1); mbar_init(&pv_empty[s], T::NWARPS); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    // ---- producer warpgroup: one lane streams every load of this CTA, then exits -------------------------------------
+    if (tid >= T::THREADS) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T::PROD_REGS));
+        if (tid != T::THREADS) return;
+        const uint64_t pol_pv = l2_policy(P.pol_pv), pol_c = l2_policy(P.pol_c), pol_h = l2_policy(P.pol_h);
+        int hs = 0, ps = 0;
+        uint32_t hph = 0, pph = 0;
+        IsoCursor pr;
+        for (pr.unit = blockIdx.x; pr.unit < nunits; pr.unit += gridDim.x) {
+            iso_unit_setup<T>(pr, P);
+            const int lx = pr.n_it - 2 * R;
+            const int cz = P.pad_z + pr.z0, cy = P.pad_y + pr.y0;
+            for (int it = 0; it < pr.n_it; it++) {
+                // plane x0 + dir*(it - R): haloed if it is computed (at step it + R), else queue-only
+                const bool halo = it >= R && it < lx + R;
+                mbar_wait(&h_empty[hs], hph ^ 1u);
+                mbar_arrive_expect_tx(&h_full[hs], halo ? T::H_BYTES : T::C_BYTES);
+                const int xp = P.pad_x + pr.x0 + pr.dir * (it - R);
+                if (halo) tma_load_3d_hint(sbase + hs * T::SLOT_BYTES, &M.h, &h_full[hs], cz - T::HZ, cy - R, xp, pol_h);
+                else tma_load_3d_hint(sbase + hs * T::SLOT_BYTES, &M.c, &h_full[hs], cz, cy, xp, pol_c);
+                if (++hs == NS) { hs = 0; hph ^= 1u; }
+                if (it >= 2 * R) {      // p(t-1) and v of the plane computed at step it
+                    const int xo = pr.x0 + pr.dir * (it - 2 * R);
+                    uint8_t* pv = sbase + T::PV_OFF + ps * T::PV_BYTES;
+                    mbar_wait(&pv_empty[ps], pph ^ 1u);
+                    mbar_arrive_expect_tx(&pv_full[ps], T::PV_BYTES);
+                    tma_load_3d_hint(pv, &M.p, &pv_full[ps], cz, cy, P.pad_x + xo, pol_pv);
+                    tma_load_3d_hint(pv + T::C_BYTES, &M.v, &pv_full[ps], P.vpad_z + pr.z0, P.vpad_y + pr.y0, P.vpad_x + xo, pol_pv);
+                    if (++ps == NPV) { ps = 0; pph ^= 1u; }
+                }
+            }
+        }
+        return;
+    }
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T::CONS_REGS));
+
+    if (P.peer_probe == 2) __nanosleep((blockIdx.x & 7u) * 2000u);
+    // ---- consumers ---------------------------------------------------------------------------------------------------
+    const int rp = tid / T::TZQ;           // row pair 0..TYP-1  (rows 2rp, 2rp+1)
+    const int quad = tid % T::TZQ;
+    const uint32_t h_own = ((2 * rp + R) * T::HP + T::HZ + 4 * quad) * ES;   // row a centre in a haloed slot
+    const uint32_t c_own = (2 * rp * T::TZ + 4 * quad) * ES;                 // row a in a halo-less slot / the p(t-1), v tiles
+
+    int hs = 0, ps = 0;
+    uint32_t hph = 0, pph = 0;
+    V qa[QL], qb[QL];
+#pragma unroll
+    for (int k = 0; k < QL; k++) { qa[k] = make_float4(0.f, 0.f, 0.f, 0.f); qb[k] = qa[k]; }
+
+    bool sig_pending = P.sig_counter != nullptr;
+    IsoCursor cu;
+    for (cu.unit = blockIdx.x; cu.unit < nunits; cu.unit += gridDim.x) {
+        if (sig_pending && cu.unit >= P.sig_units) { iso_boundary_arrive(P, lane); sig_pending = false; }   // (a CTA without boundary-first units)
+        iso_unit_setup<T>(cu, P);
+        const int lx = cu.n_it - 2 * R;
+        const int ya = cu.y0 + 2 * rp;
+        const int zq = cu.z0 + 4 * quad;
+        const int nz_ok = max(0, min(4, P.z_end - zq));
+        const int nva = (ya < P.y_end) ? nz_ok : 0;
+        const int nvb = (ya + 1 < P.y_end) ? nz_ok : 0;
+        float* out_a = P.out + (long long)ya * P.out_sy + zq + (long long)cu.x0 * P.out_sx;
+        const long long out_step = (long long)cu.dir * P.out_sx;
+        const bool vec_ok = ((reinterpret_cast<uintptr_t>(out_a) & 15) == 0);
+        const bool sig_here = sig_pending && cu.unit < P.sig_units && cu.unit + int(gridDim.x) >= P.sig_units;
+
+        // One sweep step: push plane x0 - R + it into the queues (slot hs); from step 2R on compute plane x0 + (it - 2R), whose
+        // haloed slot arrived R steps ago.  B = index of the oldest live queue entry after the push.
+        auto step = [&](auto Bc, const int it) {
+            constexpr int B = decltype(Bc)::value;
+            const bool halo = it >= R && it < lx + R;
+            const uint8_t* sl = sbase + hs * T::SLOT_BYTES;
+            mbar_wait(&h_full[hs], hph);
+            if (B == 0) {
+#pragma unroll
+                for (int k = 0; k + 2 < QL; k++) { qa[k] = qa[k + 2]; qb[k] = qb[k + 2]; }
+            }
+            const uint32_t own = halo ? h_own : c_own;
+            qa[B + QN - 1] = *reinterpret_cast<const V*>(sl + own);
+            qb[B + QN - 1] = *reinterpret_cast<const V*>(sl + own + (halo ? T::HP : T::TZ) * ES);
+
+            const bool compute = it >= 2 * R;
+            const int hc = hs >= R ? hs - R : hs - R + NS;     // slot of the plane computed now
+            if (compute) {
+                const uint8_t* pv = sbase + T::PV_OFF + ps * T::PV_BYTES;
+                mbar_wait(&pv_full[ps], pph);
+                iso_rows_update<T, MODE, B>(P, qa, qb, sbase + hc * T::SLOT_BYTES + h_own, pv + c_own, pv + T::C_BYTES + c_own,
+                                            out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb, vec_ok);
+            }
+            __syncwarp();
+            if (lane == 0) {
+                if (compute) { mbar_arrive(&pv_empty[ps]); mbar_arrive(&h_empty[hc]); }
+                if (!halo) mbar_arrive(&h_empty[hs]);
+            }
+            if (compute && ++ps == NPV) { ps = 0; pph ^= 1u; }
+            if (++hs == NS) { hs = 0; hph ^= 1u; }
+            if (sig_here && it == 3 * R - 1) { iso_boundary_arrive(P, lane); sig_pending = false; }
+        };
+        // trip = [rotate by 2, push] then [push]: the second plane lands one entry further along
+#pragma unroll 1
+        for (int it = 0; it < cu.n_it; it += 2) {
+            step(std::integral_constant<int, 0>{}, it);
+            if (it + 1 < cu.n_it) step(std::integral_constant<int, 1>{}, it + 1);
         }
     }
     if (sig_pending) iso_boundary_arrive(P, lane);
