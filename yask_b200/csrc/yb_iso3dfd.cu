@@ -76,10 +76,14 @@ void iso3dfd_coeffs(int radius, double* c) {
     for (int r = 0; r <= radius; r++) c[r] = const_roundtrip(full[radius + r]);
 }
 
-StencilSpec iso3dfd_spec(int radius, int elem_bytes, bool) {
+// sponge: iso3dfd_sponge (/root/reference/src/stencils/Iso3dfdStencil.cpp:212-249), iso3dfd with an absorbing boundary: three 1-D
+// vars cr_x(x), cr_y(y), cr_z(z) after p and v, as the generated solution declares them (no halo, not written), and
+// p(t+1) *= cr_x * cr_y * cr_z.
+StencilSpec iso3dfd_spec(int radius, int elem_bytes, bool sponge) {
     StencilSpec sp;
-    sp.name = "iso3dfd";
-    sp.description = "isotropic 3-D finite-difference wave equation, 2nd order in time, order 2*radius in space";
+    sp.name = sponge ? "iso3dfd_sponge" : "iso3dfd";
+    sp.description = sponge ? "isotropic 3-D finite-difference wave equation with an absorbing sponge boundary, order 2*radius in space"
+                            : "isotropic 3-D finite-difference wave equation, 2nd order in time, order 2*radius in space";
     sp.domain_dims = {"x", "y", "z"};
     sp.radius = radius;
     sp.elem_bytes = elem_bytes;
@@ -103,14 +107,25 @@ StencilSpec iso3dfd_spec(int radius, int elem_bytes, bool) {
         v.dims.push_back(ds);
     }
     sp.vars = {p, v};
+    if (sponge) {
+        for (int d = 0; d < 3; d++) {
+            VarSpec cr;
+            cr.name = std::string("cr_") + dn[d];
+            cr.step_alloc = 1;
+            DimSpec ds; ds.name = dn[d]; ds.kind = DIM_DOMAIN; ds.domain_index = d;
+            cr.dims.push_back(ds);
+            sp.vars.push_back(cr);
+        }
+    }
     StageSpec st;
     st.name = "stage_1";
     st.outputs = {0};
-    st.inputs = {0, 1};
-    // reference compiler counts for radius r: reads 6r+3, writes 1, fp ops 7r+5 (r=8: 51/1/61)
-    st.reads = 6 * radius + 3;
+    st.inputs = sponge ? std::vector<int>{0, 1, 2, 3, 4} : std::vector<int>{0, 1};
+    // reference compiler counts for radius r: reads 6r+3, writes 1, fp ops 7r+5 (r=8: 51/1/61); the sponge reads its three
+    // factors and multiplies by them: reads 6r+6, fp ops 7r+8 (r=8: 54/1/64, the generated part's counts)
+    st.reads = 6 * radius + (sponge ? 6 : 3);
     st.writes = 1;
-    st.fp_ops = 7 * radius + 5;
+    st.fp_ops = 7 * radius + (sponge ? 8 : 5);
     sp.stages = {st};
     return sp;
 }
@@ -260,6 +275,7 @@ __global__ void slot_box_copy_kernel(float* dst, const float* src, long long sx,
 struct IsoEngine : Engine {
     int radius = 8;
     bool f64 = false;              // 8-byte elements: the double-precision sweep (iso_radius_cfg_f64), one compiled variant per radius
+    bool sponge = false;           // iso3dfd_sponge: the SP form of the sweep (iso_sponge_cfg / iso_sponge_cfg_f64) and direct kernels
     double coef[ISO_MAX_R + 1] = {0};
     std::string kernel = "auto";   // auto | tma | direct
     int tile = DEFAULT_TILE;       // index into tile_cfg(): 16x128, producer warpgroup, 2 planes per trip
@@ -314,7 +330,7 @@ struct IsoEngine : Engine {
         else if (k == "block_steps") {
             block_steps = std::max(1, atoi(v.c_str()));
             if (!s.prepared && s.vars.size() >= 2) {
-                const bool on = block_steps >= 2 && s.spec.radius <= TT_MAX_R && s.spec.elem_bytes == 4;
+                const bool on = block_steps >= 2 && s.spec.radius <= TT_MAX_R && s.spec.elem_bytes == 4 && !is_sponge(s.spec);
                 s.vars[0].extra_slots = on ? 2 : 0;
                 if (on) {
                     // the tile's boxes reach 2R rows / planes (p) and R rows / planes, one 16-byte vector in z (v) below the
@@ -343,12 +359,19 @@ struct IsoEngine : Engine {
         return true;
     }
 
+    // iso3dfd_sponge has no temporal tile: block_steps=2 runs one step per sweep, as in fp64
+    static bool is_sponge(const StencilSpec& sp) { return sp.name == "iso3dfd_sponge"; }
+
     int prepare(Solution& s) override {
         radius = s.spec.radius;
         if (radius < 1 || radius > ISO_MAX_R) return set_error(YB_EUNSUPPORTED, "iso3dfd radius must be in 1..%d", ISO_MAX_R);
         if (s.spec.elem_bytes != 4 && s.spec.elem_bytes != 8) return set_error(YB_EUNSUPPORTED, "iso3dfd: elements must be 4 or 8 bytes");
         f64 = s.spec.elem_bytes == 8;
-        if (f64 && !iso_radius_cfg_f64(radius))
+        sponge = is_sponge(s.spec);
+        if (sponge && (f64 ? !iso_sponge_cfg_f64(radius) : !iso_sponge_cfg(radius)))
+            return set_error(YB_EUNSUPPORTED, "iso3dfd_sponge: the hand-written sweep serves radius 1-7 in fp32 and 1, 2, 3, 4, 5, 7 and 8 "
+                                              "in fp64 (fp32 radius 8 and fp64 radius 6 are generated)");
+        if (f64 && !sponge && !iso_radius_cfg_f64(radius))
             return set_error(YB_EUNSUPPORTED, "iso3dfd fp64: the hand-written sweep serves radius 1, 2, 4, 5, 6 and 7 (3 and 8 are generated)");
         iso3dfd_coeffs(radius, coef);
         cudaDeviceProp prop;
@@ -359,7 +382,7 @@ struct IsoEngine : Engine {
         const int nsl = s.vars[0].nslots();
         if (nsl > 4) return set_error(YB_EUNSUPPORTED, "iso3dfd: at most 4 storage slots of p");
         if (prop.major >= 9 && f64) {
-            const TileCfgT<double>& c = *iso_radius_cfg_f64(radius);
+            const TileCfgT<double>& c = sweep_cfg<double>();
             for (int cur = 0; cur < nsl; cur++)
                 if (int rc = make_maps(s, c, cur, maps[0][cur])) return rc;
             maps_ok = true;
@@ -368,12 +391,13 @@ struct IsoEngine : Engine {
             const Var& p = s.vars[0];
             const Var& v = s.vars[1];
             for (int tl = 0; tl < (radius == 8 ? NTILES : 1); tl++) {
-                const TileCfg& c = radius == 8 ? tile_cfg(tl) : *iso_radius_cfg(radius);
+                const TileCfg& c = radius == 8 ? tile_cfg(tl) : sweep_cfg<float>();
                 for (int cur = 0; cur < nsl; cur++)
                     if (int rc = make_maps(s, c, cur, maps[tl][cur])) return rc;
             }
             maps_ok = true;
-            if (const TTCfg* tc = (p.extra_slots == 2 && nsl == 4) ? tt_radius_cfg(radius, 0) : nullptr) {
+            // (the temporal tile computes plain iso3dfd: never for a sponge solution, whatever gave p its spare slots)
+            if (const TTCfg* tc = (p.extra_slots == 2 && nsl == 4 && !sponge) ? tt_radius_cfg(radius, 0) : nullptr) {
                 for (int cur = 0; cur < nsl; cur++) {
                     TTMaps& m = tt_maps[cur];
                     if (int rc = make_map(&m.pin, p, cur, tc->iz, tc->iy)) return rc;
@@ -388,7 +412,13 @@ struct IsoEngine : Engine {
             const TileCfg& c = sweep_cfg<float>();
             for (int m = 0; m < 4; m++) preload_kernel((const void*)c.fn[m]);
         }
-        if (f64) {
+        if (sponge) {
+            const void* fns[2][3] = {{(const void*)iso3dfd_direct_kernel<float, 0, true>, (const void*)iso3dfd_direct_kernel<float, 1, true>,
+                                      (const void*)iso3dfd_direct_kernel<float, 2, true>},
+                                     {(const void*)iso3dfd_direct_kernel<double, 0, true>, (const void*)iso3dfd_direct_kernel<double, 1, true>,
+                                      (const void*)iso3dfd_direct_kernel<double, 2, true>}};
+            for (int m = 0; m < 3; m++) preload_kernel(fns[f64][m]);
+        } else if (f64) {
             preload_kernel((const void*)iso3dfd_direct_kernel<double, 0>);
             preload_kernel((const void*)iso3dfd_direct_kernel<double, 1>);
             preload_kernel((const void*)iso3dfd_direct_kernel<double, 2>);
@@ -412,11 +442,12 @@ struct IsoEngine : Engine {
     }
 
     // The sweep variant a launch uses: the selected tile (in its resident-plane form where it has one and `resident` is on) at
-    // radius 8, the one compiled variant at other radii.
-    bool resident_on() const { return radius == 8 && !f64 && resident && resident_cfg(tile); }
+    // radius 8, the one compiled variant at other radii, in fp64 and for iso3dfd_sponge (which has no fp32 radius-8 form).
+    bool resident_on() const { return radius == 8 && !f64 && !sponge && resident && resident_cfg(tile); }
     template <class E>
     const TileCfgT<E>& sweep_cfg() const {
-        if constexpr (sizeof(E) == 8) return *iso_radius_cfg_f64(radius);
+        if constexpr (sizeof(E) == 8) return sponge ? *iso_sponge_cfg_f64(radius) : *iso_radius_cfg_f64(radius);
+        else if (sponge) return *iso_sponge_cfg(radius);
         else return radius != 8 ? *iso_radius_cfg(radius) : resident_on() ? *resident_cfg(tile) : tile_cfg(tile);
     }
     // Row of attr_set: the tile at radius 8 (NTILES + 0 / 1: resident forms of tiles 6 / 7), 0 otherwise.
@@ -444,6 +475,12 @@ struct IsoEngine : Engine {
         P.vpad_x = int(vx->pad_l); P.vpad_y = int(vy->pad_l); P.vpad_z = int(vz->pad_l);
         P.pol_c = pol_c; P.pol_h = pol_h; P.pol_pv = pol_pv; P.st_cs = st_cs; P.peer_probe = peer_probe;
         for (int r = 0; r <= ISO_MAX_R; r++) P.c[r] = r <= radius ? E(coef[r]) : E(0);    // fp64: the round-tripped doubles as they are
+        P.cr_x = P.cr_y = P.cr_z = nullptr;
+        if (sponge) {       // vars 2, 3, 4: cr_x, cr_y, cr_z, each at its domain origin
+            P.cr_x = reinterpret_cast<const E*>(s.vars[2].slot_ptr(0)) + s.vars[2].origin_offset();
+            P.cr_y = reinterpret_cast<const E*>(s.vars[3].slot_ptr(0)) + s.vars[3].origin_offset();
+            P.cr_z = reinterpret_cast<const E*>(s.vars[4].slot_ptr(0)) + s.vars[4].origin_offset();
+        }
     }
 
     int launch(Solution& s, int, int64_t t, const Box& box, cudaStream_t st) override {
@@ -470,7 +507,7 @@ struct IsoEngine : Engine {
             use_tma = false;
         }
         if (use_tma) {
-            const int ti = radius == 8 ? tile : 0;      // tensor maps; other radii and fp64: one compiled variant
+            const int ti = (radius == 8 && !f64 && !sponge) ? tile : 0;      // tensor maps; other radii, fp64 and sponge: one compiled variant
             const int ai = cfg_index();
             const TileCfgT<E>& c = sweep_cfg<E>();
             if (mem_probe && c.fn[3]) mode = 3;
@@ -550,10 +587,18 @@ struct IsoEngine : Engine {
             dim3 blk(128, 1, 1);
             dim3 grd(unsigned((box.e[2] - box.b[2] + 127) / 128), unsigned(box.e[1] - box.b[1]), unsigned(box.e[0] - box.b[0]));
             if (grd.y > 65535 || grd.z > 65535) return set_error(YB_EUNSUPPORTED, "direct kernel: domain too large in x or y");
-            switch (mode) {
-                case 0: iso3dfd_direct_kernel<E, 0><<<grd, blk, 0, st>>>(P, radius); break;
-                case 1: iso3dfd_direct_kernel<E, 1><<<grd, blk, 0, st>>>(P, radius); break;
-                default: iso3dfd_direct_kernel<E, 2><<<grd, blk, 0, st>>>(P, radius); break;
+            if (sponge) {
+                switch (mode) {
+                    case 0: iso3dfd_direct_kernel<E, 0, true><<<grd, blk, 0, st>>>(P, radius); break;
+                    case 1: iso3dfd_direct_kernel<E, 1, true><<<grd, blk, 0, st>>>(P, radius); break;
+                    default: iso3dfd_direct_kernel<E, 2, true><<<grd, blk, 0, st>>>(P, radius); break;
+                }
+            } else {
+                switch (mode) {
+                    case 0: iso3dfd_direct_kernel<E, 0><<<grd, blk, 0, st>>>(P, radius); break;
+                    case 1: iso3dfd_direct_kernel<E, 1><<<grd, blk, 0, st>>>(P, radius); break;
+                    default: iso3dfd_direct_kernel<E, 2><<<grd, blk, 0, st>>>(P, radius); break;
+                }
             }
         }
         YB_CUDA(cudaGetLastError());
@@ -658,7 +703,7 @@ struct IsoEngine : Engine {
     // In-run tuner: the same variants as the offline tuner, one per step of a live run.
     static constexpr int TUNE_TILES[6] = {7, 6, 5, 4, 1, 0};
     static constexpr int TUNE_LXS[3] = {0, 256, 512};
-    int tune_variants(const Solution&) const override { return (maps_ok && radius == 8 && kernel != "direct") ? 18 : 0; }
+    int tune_variants(const Solution&) const override { return (maps_ok && radius == 8 && !f64 && !sponge && kernel != "direct") ? 18 : 0; }
     void tune_select(Solution& s, int v) override {
         tile = TUNE_TILES[v / 3]; lx = TUNE_LXS[v % 3];
         s.options["tile"] = std::to_string(tile);
@@ -709,7 +754,8 @@ struct IsoEngine : Engine {
     // Offline tuner: the compiled sweep variants (tile shape, producer warpgroup, planes per trip, resident planes) x sweep
     // chunk lengths, timed over the whole rank box; the analogue of the reference's block-size search
     // (/root/reference/src/kernel/lib/auto_tuner.cpp) for the knobs this engine has.  fp64 has one variant per radius: only
-    // the chunk length is searched.
+    // the chunk length is searched.  iso3dfd_sponge keeps the same behaviour: fp64 searches the chunk length, fp32 (radius 1-7)
+    // has nothing to tune.
     int auto_tune(Solution& s, cudaStream_t st, std::string& report) override {
         if (tt_ok && kernel != "direct" && !s.multi_rank()) return auto_tune_temporal(s, st, report);
         if (!maps_ok || (radius != 8 && !f64) || kernel == "direct") { report = "iso3dfd: no tiled variants to tune for this configuration"; return 0; }
@@ -736,7 +782,7 @@ struct IsoEngine : Engine {
                 int64_t t = t0;
                 const double ms = time_launches(st, 3, [&]() { return launch(s, 0, t++, whole, st); });
                 if (ms < 0) { tile = keep_tile; resident = keep_res; lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-                snprintf(line, sizeof line, " tile=%d resident=%d (%s) lx=%d: %.4f ms/step\n", ti, int(resident_on()), f64 ? iso_radius_cfg_f64(radius)->name : sweep_cfg<float>().name, l, ms);
+                snprintf(line, sizeof line, " tile=%d resident=%d (%s) lx=%d: %.4f ms/step\n", ti, int(resident_on()), f64 ? sweep_cfg<double>().name : sweep_cfg<float>().name, l, ms);
                 report += line;
                 if (ms < best) { best = ms; best_tile = ti; best_res = res; best_lx = l; }
             }

@@ -73,6 +73,12 @@ struct IsoParamsT {
     unsigned long long* sig_flag_hi;
     unsigned long long sig_epoch;
     E c[ISO_MAX_R + 1];
+    // iso3dfd_sponge (the kernels' SP form): element 0 of the rank domain of the 1-D vars cr_x(x), cr_y(y), cr_z(z).  Their
+    // unit-stride dim is padded like every var's, so cr_z's origin sits on a 128-byte boundary and its alloc is a whole number
+    // of 16-byte vectors.
+    const E* cr_x;
+    const E* cr_y;
+    const E* cr_z;
 };
 using IsoParams = IsoParamsT<float>;
 
@@ -80,8 +86,16 @@ using IsoParams = IsoParamsT<float>;
 // Reference-order direct kernel: one thread per point, straight global loads (through L1/L2).
 // Used for radii/shapes the tiled kernel does not cover and as the on-device cross-check of the
 // tiled kernel at sizes the CPU oracle cannot reach.  Any radius 1..8.
+// SP: iso3dfd_sponge, p(t+1) *= cr_x(x) * cr_y(y) * cr_z(z) in the reference's statement order
+// (/root/reference/src/stencils/Iso3dfdStencil.cpp:212-249): three rounded multiplies, ((p * cr_x) * cr_y) * cr_z, never the
+// product of the three factors first (its rounding differs).  No addition follows them, so they are the same in every FP mode.
 // ---------------------------------------------------------------------------------------------
-template <class E, int MODE>
+template <class E>
+__device__ __forceinline__ E iso_sponge(E p, E crx, E cry, E crz) {
+    return iso_mul(iso_mul(iso_mul(p, crx), cry), crz);
+}
+
+template <class E, int MODE, bool SP = false>
 __global__ void __launch_bounds__(256) iso3dfd_direct_kernel(IsoParamsT<E> P, int R) {
     const int z = P.z_begin + blockIdx.x * blockDim.x + threadIdx.x;
     const int y = P.y_begin + blockIdx.y;
@@ -96,7 +110,9 @@ __global__ void __launch_bounds__(256) iso3dfd_direct_kernel(IsoParamsT<E> P, in
                               pc[r * P.out_sy], pc[-r], pc[r], r == 1);
     }
     const E v = P.vel[(long long)x * P.v_sx + (long long)y * P.v_sy + z];
-    P.out[o] = iso_final<MODE>(acc, center, P.prev[o], v);
+    const E r = iso_final<MODE>(acc, center, P.prev[o], v);
+    if constexpr (SP) P.out[o] = iso_sponge(r, P.cr_x[x], P.cr_y[y], P.cr_z[z]);
+    else P.out[o] = r;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -196,9 +212,10 @@ struct IsoTile2 {
     static_assert(C_BYTES % 128 == 0, "TMA destination alignment");
 };
 
-// Boundary-phase completion (see IsoParams::sig_*): called once per consumer warp, by all of its lanes.
+// Boundary-phase completion (see IsoParams::sig_*): called once per consumer warp, by all of its lanes.  Out of line in the
+// plain sweep; the sponge form (SP) inlines it, since the registers live across the call spilled there.
 template <class PT>
-__device__ __noinline__ void iso_boundary_arrive(const PT& P, int lane) {
+__device__ __forceinline__ void iso_boundary_arrive_inl(const PT& P, int lane) {
     __threadfence_system();          // this lane's peer stores are ordered before what follows, at system scope
     __syncwarp();
     if (lane == 0) {
@@ -211,6 +228,8 @@ __device__ __noinline__ void iso_boundary_arrive(const PT& P, int lane) {
         }
     }
 }
+template <class PT>
+__device__ __noinline__ void iso_boundary_arrive(const PT& P, int lane) { iso_boundary_arrive_inl(P, lane); }
 
 __device__ __forceinline__ void f4_to_arr(const float4& v, float* a) { a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w; }
 __device__ __forceinline__ void f4_to_arr(const double2& v, double* a) { a[0] = v.x; a[1] = v.y; }
@@ -226,10 +245,20 @@ __device__ __forceinline__ void arr_to_v(const double* a, double2& v) { v = make
 // Results leave as 128-bit stores where the row's vector is whole and aligned (scalars on ragged edges).  The fused halo
 // exchange (peer stores into the x neighbours' halo cells) is compiled for fp32 only: the fp64 sweep is listed with
 // fused_ok = false, and leaving the out-of-line signal call out keeps its registers free of call spills.
-template <class T, int MODE, int B, int QL>
+// SP (iso3dfd_sponge): both rows' results are scaled by the sponge factors in `sg` (iso_sponge) before every store, the peer
+// stores included.
+template <class E>
+struct IsoSpongeRegs {
+    E x;                    // cr_x of the plane computed now
+    E ya, yb;               // cr_y of rows a and b
+    E z[IsoVec<E>::N];      // cr_z of the thread's vector
+};
+
+template <class T, int MODE, int B, int QL, bool SP = false>
 __device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>& P, const typename T::V (&qa)[QL],
                                                 const typename T::V (&qb)[QL], const uint8_t* h, const uint8_t* pv,
-                                                const uint8_t* v, typename T::E* oa, int xo, int nva, int nvb, bool vec_ok) {
+                                                const uint8_t* v, typename T::E* oa, int xo, int nva, int nvb, bool vec_ok,
+                                                const IsoSpongeRegs<typename T::E>* sg = nullptr) {
     using E = typename T::E;
     using V = typename T::V;
     constexpr int R = T::R, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
@@ -291,6 +320,13 @@ __device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>&
         for (int i = 0; i < VW; i++) ea[i] = iso_final<MODE>(acca[i], pa[i], pva[i], vva[i]);
 #pragma unroll
         for (int i = 0; i < VW; i++) eb[i] = iso_final<MODE>(accb[i], pb[i], pvb[i], vvb[i]);
+        if constexpr (SP) {
+#pragma unroll
+            for (int i = 0; i < VW; i++) {
+                ea[i] = iso_sponge(ea[i], sg->x, sg->ya, sg->z[i]);
+                eb[i] = iso_sponge(eb[i], sg->x, sg->yb, sg->z[i]);
+            }
+        }
         V ra, rb;
         arr_to_v(ea, ra); arr_to_v(eb, rb);
         E* ob = oa + P.out_sy;
@@ -327,7 +363,9 @@ __device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>&
 //         issue code (with 2 warps per scheduler a straggling warp 0 delays every stage hand-over).
 // U  = 2: the sweep loop handles two planes per trip and rotates the x queues by two entries every second
 //         plane (half the register moves of U = 1) at the price of one extra queue entry per row.
-template <class T, int MODE, int PW = 0, int U = 1>
+// SP = true: iso3dfd_sponge.  The sponge factors live in registers: cr_z (one 16-byte vector) and cr_y (two rows) are loaded
+//         once per work unit, cr_x one plane ahead of the plane it scales, in the chunk's sweep direction.
+template <class T, int MODE, int PW = 0, int U = 1, bool SP = false>
 __global__ void __launch_bounds__(T::THREADS + 128 * PW, 1)
 iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ IsoParamsT<typename T::E> P) {
     using E = typename T::E;
@@ -335,6 +373,10 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
     constexpr int R = T::R, QN = T::QN, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
     constexpr int QL = QN + (U - 1);          // queue entries kept per row
     constexpr bool FUSED = sizeof(E) == 4;    // see iso_rows_update
+    // setmaxnreg split: the fp32 sponge form gives its producer warpgroup 32 registers (at 24 it spilled at radius 1-4), which
+    // leaves its consumers 232 of the 168 x 384 the CTA is launched with
+    constexpr int PROD_REGS = (SP && FUSED) ? 32 : T::PROD_REGS;
+    constexpr int CONS_REGS = (SP && FUSED) ? 232 : T::CONS_REGS;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     uint8_t* sbase = smem_raw + (base - smem_u32(smem_raw));
@@ -384,11 +426,11 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
         // Warp-specialised register budget (setmaxnreg works on whole warpgroups): the producer warpgroup
         // hands its registers back, the two consumer warpgroups take them.
         if (tid >= T::THREADS) {          // producer warpgroup: one lane streams every load of this CTA, then exits
-            asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T::PROD_REGS));
+            asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
             while (pr_live) produce_one();
             return;
         }
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T::CONS_REGS));
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
     } else if (tid == 0) {
         for (int k = 0; k < T::STAGES - 1 && pr_live; k++) produce_one();
     }
@@ -407,8 +449,9 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
     for (int k = 0; k < QL; k++) { const E zero[VW] = {}; arr_to_v(zero, qa[k]); qb[k] = qa[k]; }
 
     bool sig_pending = FUSED && P.sig_counter != nullptr;
+    auto arrive = [&]() { if constexpr (SP) iso_boundary_arrive_inl(P, lane); else iso_boundary_arrive(P, lane); };
     for (cu.unit = blockIdx.x; cu.unit < nunits; cu.unit += gridDim.x) {
-        if (sig_pending && cu.unit >= P.sig_units) { iso_boundary_arrive(P, lane); sig_pending = false; }   // (a CTA without boundary-first units)
+        if (sig_pending && cu.unit >= P.sig_units) { arrive(); sig_pending = false; }   // (a CTA without boundary-first units)
         iso_unit_setup<T>(cu, P);
         const int ya = cu.y0 + 2 * rp;
         const int zq = cu.z0 + VW * quad;
@@ -420,6 +463,20 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(out_a) & 15) == 0);
         // this warp's boundary planes are complete after plane R-1 of its last boundary-first unit
         const bool sig_here = sig_pending && cu.unit < P.sig_units && cu.unit + int(gridDim.x) >= P.sig_units;
+        IsoSpongeRegs<E> sg;
+        [[maybe_unused]] E crx_next;       // cr_x of the next plane to compute
+        if constexpr (SP) {
+            // zq < z_end keeps the vector inside cr_z's allocation (whole 16-byte vectors from a 128-byte aligned origin); a
+            // thread without points in z takes ones
+            if (nz_ok > 0) f4_to_arr(*reinterpret_cast<const V*>(P.cr_z + zq), sg.z);
+            else {
+#pragma unroll
+                for (int i = 0; i < VW; i++) sg.z[i] = E(1);
+            }
+            sg.ya = nva > 0 ? P.cr_y[ya] : E(1);
+            sg.yb = nvb > 0 ? P.cr_y[ya + 1] : E(1);
+            crx_next = P.cr_x[cu.x0];
+        }
 
         // One sweep step.  B = index of the oldest live queue entry after the push (window = q[B .. B+2R]).
         auto step = [&](auto Bc, const int it) {
@@ -437,13 +494,19 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
             qa[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own);
             qb[B + QN - 1] = *reinterpret_cast<const V*>(st + T::C_OFF + c_own + T::TZ * ES);
 
-            if (it >= 2 * R)
-                iso_rows_update<T, MODE, B>(P, qa, qb, st + T::H_OFF + h_own, st + T::P_OFF + c_own, st + T::V_OFF + c_own,
-                                            out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb, vec_ok);
+            if (it >= 2 * R) {
+                if constexpr (SP) {
+                    sg.x = crx_next;
+                    if (it + 1 < cu.n_it) crx_next = P.cr_x[cu.x0 + cu.dir * (it + 1 - 2 * R)];   // used at the next step
+                }
+                iso_rows_update<T, MODE, B, QL, SP>(P, qa, qb, st + T::H_OFF + h_own, st + T::P_OFF + c_own, st + T::V_OFF + c_own,
+                                                    out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb,
+                                                    vec_ok, &sg);
+            }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[cu.stage]);
             if (++cu.stage == T::STAGES) { cu.stage = 0; cu.phase ^= 1u; }
-            if (sig_here && it == 3 * R - 1) { iso_boundary_arrive(P, lane); sig_pending = false; }
+            if (sig_here && it == 3 * R - 1) { arrive(); sig_pending = false; }
         };
 
         if (U == 1) {
@@ -458,7 +521,7 @@ iso3dfd_tma2_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
             }
         }
     }
-    if (sig_pending) iso_boundary_arrive(P, lane);
+    if (sig_pending) arrive();
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -24,4 +24,9 @@ const TileCfg* iso_radius_cfg(int radius);
 // and 8 are served by the emitter-generated kernels (yb_stencils.cpp), so they have no entry here: returns nullptr.
 const TileCfgT<double>* iso_radius_cfg_f64(int radius);
 
+// iso3dfd_sponge (yb_iso3dfd_sponge.cu): the same default variant in its SP form, fp32 at radius 1..7 and fp64 at radius 1, 2, 3,
+// 4, 5, 7 and 8.  fp32 radius 8 and fp64 radius 6 are served by the emitter-generated kernels (yb_stencils.cpp): nullptr.
+const TileCfg* iso_sponge_cfg(int radius);
+const TileCfgT<double>* iso_sponge_cfg_f64(int radius);
+
 }  // namespace yb

@@ -40,12 +40,23 @@ int registry_create(const std::string& name, int radius, int elem_bytes, Stencil
         eng = make_iso3dfd_engine();
         return 0;
     }
-    if (name == "iso3dfd_sponge" && elem_bytes == 8) {
-        // fp64: generated for radius 6, the reference's fp64 validation run of this solution (src/kernel/Makefile:1156)
-        if (radius > 0 && radius != 6) return set_error(YB_EUNSUPPORTED, "iso3dfd_sponge fp64 is generated for radius 6 only");
-        int rc = gen_registry_create("iso3dfd_sponge_fp64_r6", 8, spec, eng);
-        if (rc == 0) { spec.name = "iso3dfd_sponge"; spec.radius = 6; }
-        return rc;
+    if (name == "iso3dfd_sponge") {
+        // Its default radius in each precision stays on the emitter-generated kernels: 8 in fp32, and in fp64 6, the reference's
+        // fp64 validation run of this solution (src/kernel/Makefile:1156).  Every other radius up to 8 takes the hand-written
+        // iso3dfd sweep in its sponge form.
+        const bool f64 = elem_bytes == 8;
+        if (radius > 8) return set_error(YB_EUNSUPPORTED, "iso3dfd_sponge: radius %d > 8 is not supported", radius);
+        if (radius <= 0 || radius == (f64 ? 6 : 8)) {
+            if (!f64) return gen_registry_create(name, elem_bytes, spec, eng);
+            int rc = gen_registry_create("iso3dfd_sponge_fp64_r6", 8, spec, eng);
+            if (rc == 0) { spec.name = "iso3dfd_sponge"; spec.radius = 6; }
+            return rc;
+        }
+        if (elem_bytes == 0) elem_bytes = 4;
+        if (elem_bytes != 4 && elem_bytes != 8) return set_error(YB_EUNSUPPORTED, "iso3dfd_sponge: elements must be 4 or 8 bytes");
+        spec = iso3dfd_spec(radius, elem_bytes, true);
+        eng = make_iso3dfd_engine();
+        return 0;
     }
     int rc = gen_registry_create(name, elem_bytes, spec, eng);
     if (rc != YB_EINVAL) return rc;

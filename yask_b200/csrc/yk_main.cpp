@@ -127,9 +127,11 @@ int main(int argc, char** argv) {
         for (auto& v : soln->get_vars()) v->set_all_elements_same(var_val(k++));
 
         // iso3dfd runs on the hand-written engine (option -kernel) in fp32 and, in fp64, at the radii its fp64 sweep serves;
-        // fp64 at radius 3 and 8 is emitter-generated
-        bool hand_iso = soln->get_name() == "iso3dfd";
-        if (validate && hand_iso && soln->get_element_bytes() == 8) {
+        // fp64 at radius 3 and 8 is emitter-generated.  iso3dfd_sponge runs on it too, except at its default radius (8 in fp32, 6 in
+        // fp64); the hand-written engine is the one that takes option -kernel.
+        const bool sponge = soln->get_name() == "iso3dfd_sponge";
+        bool hand_iso = soln->get_name() == "iso3dfd" || sponge;
+        if (validate && hand_iso && (soln->get_element_bytes() == 8 || sponge)) {
             try {
                 kfac.new_solution(env, soln)->apply_command_line_options("-kernel direct");
             } catch (yask_exception&) {
@@ -224,6 +226,27 @@ int main(int argc, char** argv) {
             other->prepare_solution();
             k = 0;
             for (auto& v : other->get_vars()) v->set_all_elements_same(var_val(k++));
+            // iso3dfd_sponge: a ripple in [0.95, 1] along each sponge factor (a function of the global index, the same in both
+            // solutions), so that a factor taken from the wrong row, plane or vector shows up -- constant factors would only
+            // check the rounding order of the three multiplies
+            if (sponge) {
+                for (const char* name : {"cr_x", "cr_y", "cr_z"}) {
+                    yk_var_ptr vars[2] = {soln->get_var(name), other->get_var(name)};
+                    const std::string d = vars[0]->get_dim_names()[0];
+                    const idx_t_vec f{vars[0]->get_first_rank_domain_index(d)}, l{vars[0]->get_last_rank_domain_index(d)};
+                    const size_t n = size_t(l[0] - f[0] + 1);
+                    std::vector<double> bd(n);
+                    std::vector<float> bf(n);
+                    for (size_t i = 0; i < n; i++) {
+                        bd[i] = 0.95 + 0.05 * double((f[0] + idx_t(i)) * 7919 % 101) / 100.0;
+                        bf[i] = float(bd[i]);
+                    }
+                    for (auto& v : vars) {
+                        if (soln->get_element_bytes() == 8) v->set_elements_in_slice(bd.data(), n, f, l);
+                        else v->set_elements_in_slice(bf.data(), n, f, l);
+                    }
+                }
+            }
             // a bump in the middle so that the field is not constant
             idx_t_vec mid;
             mid.push_back(0);
