@@ -415,7 +415,7 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     if (s->prepared) return 0;
     if (int rc = compute_rank_geometry(*s)) return rc;
     for (auto& v : s->vars) compute_var_geometry(*s, v);
-    return 0;
+    return s->engine->check_geometry(*s);
 }
 
 int yb_solution_prepare(yb_solution* s_, int device) {
@@ -426,6 +426,10 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (ndev <= 0) return set_error(YB_ECUDA, "no CUDA device available: the yask_b200 engine has no CPU fallback");
     if (device < 0 || device >= ndev) return set_error(YB_EINVAL, "device %d out of range [0,%d)", device, ndev);
     if (int rc = compute_rank_geometry(*s)) return rc;
+    // a size the kernels cannot address is refused before any storage is allocated
+    for (auto& v : s->vars)
+        if (!v.dev) compute_var_geometry(*s, v);
+    if (int rc = s->engine->check_geometry(*s)) return rc;
     YB_CUDA(cudaSetDevice(device));
     s->device = device;
     if (!s->own_stream) YB_CUDA(cudaStreamCreateWithFlags(&s->own_stream, cudaStreamNonBlocking));

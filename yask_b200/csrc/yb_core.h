@@ -132,6 +132,9 @@ struct Solution;
 // One implementation per stencil family: owns kernels, tensor maps and launch logic.
 struct Engine {
     virtual ~Engine() {}
+    // called by plan_geometry() and by prepare() once the vars' geometry is known and before any storage is allocated:
+    // refuse a size the engine's kernels cannot address.  Default: no limit.
+    virtual int check_geometry(const Solution&) const { return 0; }
     // called at the end of prepare(): build tensor maps etc.
     virtual int prepare(Solution& s) = 0;
     // launch stage `stage` of step t (computing t+1) over `box` on `stream`; returns #kernels launched or <0

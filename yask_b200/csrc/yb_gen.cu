@@ -78,6 +78,7 @@ struct GenEngine : Engine {
         for (auto& kv : sweep_maps) cudaFree(kv.second);
         sweep_maps.clear();
     }
+    bool wide = false;   // kernels in their 64-bit addressing form (prepare)
     int l2_mb = 16;    // option gen_l2_mb (env YB_GEN_L2_MB): L2 budget of one y chunk's sweep working set (0 = no chunking)
     int set_option(Solution&, const std::string& key, const std::string& value) override {
         if (key == "gen_pf") { pf_dist = std::max(0, atoi(value.c_str())); return 0; }
@@ -91,14 +92,19 @@ struct GenEngine : Engine {
         if (cudaGetDeviceProperties(&prop, s.device) == cudaSuccess) num_sms = prop.multiProcessorCount;
         if (s.spec.elem_bytes != g.elem_bytes)
             return set_error(YB_EUNSUPPORTED, "solution '%s' was generated for %d-byte elements", g.name.c_str(), g.elem_bytes);
+        // the kernels' addressing form (GenFnPair): 64-bit element positions once a var slot holds 2^31 elements or
+        // more, the 32-bit form below that (scratch vars share the solution's geometry, so the API-visible vars decide)
+        wide = false;
+        for (auto& v : s.vars) wide = wide || v.slot_elems >= (int64_t(1) << 31);
+        sweep_launches = 0;
         for (auto& st : g.stages)
             for (auto& p : st.parts)
                 if (int(p.acc.size()) > GEN_MAX_ACC) return set_error(YB_EUNSUPPORTED, "part '%s' touches too many vars", p.name);
         for (auto& st : g.stages)
             for (auto& p : st.parts)
                 for (int m = 0; m < 2; m++) {
-                    preload_kernel((const void*)p.fn[g.elem_bytes == 8 ? 1 : 0][m]);
-                    preload_kernel((const void*)p.sweep.fn[g.elem_bytes == 8 ? 1 : 0][m]);
+                    preload_kernel((const void*)p.fn[g.elem_bytes == 8 ? 1 : 0][m].pick(wide));
+                    preload_kernel((const void*)p.sweep.fn[g.elem_bytes == 8 ? 1 : 0][m].pick(wide));
                 }
         for (auto& v : scratch)
             if (v.dev) cudaFree(v.dev);
@@ -116,6 +122,60 @@ struct GenEngine : Engine {
             scratch.push_back(std::move(v));
         }
         return 0;
+    }
+    // Sizes the generated kernels cannot address, refused before anything is allocated (Engine::check_geometry):
+    //  * a dimension: launch boxes and point coordinates are int (GenParams::xb..ze, GEN_KERNEL_BEGIN), so a domain dim and
+    //    its pads must span fewer than 2^31 elements -- what bounds a 1-D solution, or the unit-stride dim of a 2-D one;
+    //  * the neighbour offsets: the kernels form each point's position in 64 bits where the slots need it, but add the
+    //    offsets dx*SX + dy*SY + dz (int SX, SY: GenParams) in 32 bits (yb_gen.cuh, GEN_POS).  |dy*SY + dz| < SX, so
+    //    (x halo + 1) x-planes of a 3-D var must stay below 2^31 elements: that bounds the y*z extent, not the size of a var;
+    //  * the launch grids: one 1-D grid per part, fewer than 2^31 CTAs (direct kernels, and sweep kernels at their longest
+    //    chunking, one plane per chunk).
+    int check_geometry(const Solution& s) const override {
+        const int64_t lim = int64_t(1) << 31;
+        const int sh = 3 - s.ndd;
+        int64_t ext[3] = {1, 1, 1};   // per kernel slot: largest extent of any var, pads included
+        for (auto& v : s.vars)
+            for (auto& d : v.dims) {
+                if (d.spec.kind != DIM_DOMAIN) continue;
+                if (d.alloc >= lim)
+                    return set_error(YB_EUNSUPPORTED,
+                                     "var '%s': dim '%s' spans %lld elements with its pads (domain %lld); the generated kernels "
+                                     "index a dimension with 32-bit ints, limit 2^31 - 1 elements",
+                                     v.spec.name.c_str(), d.spec.name.c_str(), (long long)d.alloc, (long long)d.domain);
+                ext[d.spec.domain_index + sh] = std::max(ext[d.spec.domain_index + sh], d.alloc);
+            }
+        if (s.ndd == 3)
+            for (auto& v : s.vars) {
+                const Dim* d0 = v.domain_dim(0);
+                if (!d0 || !v.domain_dim(1) || !v.domain_dim(2)) continue;
+                const int64_t reach = std::max(d0->pad_l, d0->pad_r) + 1;
+                if (reach * d0->stride >= lim)
+                    return set_error(YB_EUNSUPPORTED,
+                                     "var '%s': %lld x-planes of %lld elements (x halo + 1) reach 2^31 elements, the limit of the "
+                                     "generated kernels' 32-bit neighbour offsets; reduce the y*z extent (%lld x %lld)",
+                                     v.spec.name.c_str(), (long long)reach, (long long)d0->stride,
+                                     (long long)v.domain_dim(1)->domain, (long long)v.domain_dim(2)->domain);
+            }
+        auto cdiv = [](int64_t a, int64_t b) { return (a + b - 1) / b; };
+        const int64_t direct = cdiv(ext[2], GEN_BZ) * cdiv(ext[1], GEN_BY * gen_np(g.elem_bytes)) * cdiv(ext[0], GEN_BX);
+        int64_t grid = direct;
+        for (auto& st : g.stages)
+            for (auto& p : st.parts)
+                if (p.sweep.ty > 0 && p.sweep.tz > 0)
+                    grid = std::max(grid, cdiv(ext[2], p.sweep.tz) * cdiv(ext[1], p.sweep.ty) * ext[0]);
+        if (grid >= lim)
+            return set_error(YB_EUNSUPPORTED, "domain %lld x %lld x %lld (pads included) needs a launch grid of %lld CTAs; the "
+                             "generated kernels' 1-D grids take fewer than 2^31", (long long)ext[0], (long long)ext[1],
+                             (long long)ext[2], (long long)grid);
+        return 0;
+    }
+    // Read-only option gen_sweep_launches: sweep-kernel launches since prepare (which parts took the TMA sweep form).
+    int64_t sweep_launches = 0;
+    bool get_option(const Solution&, const std::string& key, std::string& v) const override {
+        if (key != "gen_sweep_launches") return false;
+        v = std::to_string(sweep_launches);
+        return true;
     }
     // In-run tuner: sweep kernels with the cost-model chunking or fixed chunk lengths, and the direct kernels.
     int tune_variants(const Solution&) const override { return 4; }
@@ -221,7 +281,7 @@ struct GenEngine : Engine {
                     if (d.spec.kind == DIM_DOMAIN) { in_order = in_order && d.spec.domain_index > last_di; last_di = d.spec.domain_index; }
                 if (d0 && d1 && d2 && in_order) {
                     if (P.SX == 0) { P.SX = int(d0->stride); P.SY = int(d1->stride); }
-                    if (d0->stride != P.SX || d1->stride != P.SY || d2->stride != 1 || v.slot_elems >= (int64_t(1) << 31))
+                    if (d0->stride != P.SX || d1->stride != P.SY || d2->stride != 1)
                         return set_error(YB_EUNSUPPORTED, "var '%s' does not share the solution's padded geometry", v.spec.name.c_str());
                 }
             }
@@ -237,7 +297,7 @@ struct GenEngine : Engine {
             // Sweep variant: TMA-staged shared-memory planes (yb_gen_sweep.cuh), for whole-box launches of parts that have one.
             const int fi = g.elem_bytes == 8 ? 1 : 0, mi = s.fp_mode == 0 ? 0 : 1;
             // (TMA boxes and the consumers' 128-bit accesses need the box to start on a 16-byte boundary in z)
-            if (sweep && p.sweep.fn[fi][mi] && P.SX != 0 && pb.e[0] - pb.b[0] >= sweep_min_x && pb.e[2] - pb.b[2] >= 32 &&
+            if (sweep && p.sweep.fn[fi][mi].narrow && P.SX != 0 && pb.e[0] - pb.b[0] >= sweep_min_x && pb.e[2] - pb.b[2] >= 32 &&
                 pb.b[2] % (16 / g.elem_bytes) == 0) {
                 GenSweepParams SP;
                 memset(&SP, 0, sizeof SP);
@@ -290,7 +350,7 @@ struct GenEngine : Engine {
                     SP.lx = int(best_l);
                 }
                 SP.nchunks = int((nxb + SP.lx - 1) / SP.lx);
-                GenSweepFn sfn = sw.fn[fi][mi];
+                GenSweepFn sfn = sw.fn[fi][mi].pick(wide);
                 if (!sweep_attr[(const void*)sfn]) {
                     YB_CUDA(cudaFuncSetAttribute((const void*)sfn, cudaFuncAttributeMaxDynamicSharedMemorySize, sw.smem));
                     sweep_attr[(const void*)sfn] = true;
@@ -299,6 +359,7 @@ struct GenEngine : Engine {
                 if (nb >= (int64_t(1) << 31)) return set_error(YB_EUNSUPPORTED, "domain too large for the sweep kernels");
                 sfn<<<unsigned(nb), sw.threads, sw.smem, st>>>(SP);
                 YB_CUDA(cudaGetLastError());
+                sweep_launches++;
                 n++;
                 continue;
             }
@@ -314,7 +375,7 @@ struct GenEngine : Engine {
                     if (!dup) P.pf[P.npf++] = (unsigned char)k;
                 }
             }
-            GenKernelFn fn = p.fn[g.elem_bytes == 8 ? 1 : 0][s.fp_mode == 0 ? 0 : 1];
+            GenKernelFn fn = p.fn[g.elem_bytes == 8 ? 1 : 0][s.fp_mode == 0 ? 0 : 1].pick(wide);
             const int rows_per_block = GEN_BY * gen_np(g.elem_bytes);
             P.nzb = int((pb.e[2] - pb.b[2] + GEN_BZ - 1) / GEN_BZ);
             P.nyb = int((pb.e[1] - pb.b[1] + rows_per_block - 1) / rows_per_block);

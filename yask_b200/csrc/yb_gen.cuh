@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace yb { namespace gen {
@@ -47,13 +48,23 @@ struct GenParams {
 };
 
 typedef void (*GenKernelFn)(const GenParams);
+// Generated kernels come in two addressing forms (template argument MODE | GEN_WIDE): 32-bit element positions, and 64-bit ones
+// for slots of 2^31 elements or more.  The 32-bit form is what most sizes run: in the direct kernels the 64-bit one keeps a
+// 64-bit base per var live (up to 44 more registers in the kernels of many-var parts), in the sweep kernels it costs the output
+// stores an instruction (awp_elastic 0.5 % at 512^3).  yb_gen.cu picks the form from the slots' size.
+constexpr int GEN_WIDE = 2;
+template <typename F> struct GenFnPair {
+    F narrow = nullptr, wide = nullptr;
+    F pick(bool w) const { return w ? wide : narrow; }
+};
+typedef GenFnPair<GenKernelFn> GenKernelPair;
 
 // Sweep variant (yb_gen_sweep.cuh): host-side description of one part's TMA streams; empty when the part has none.
 struct GenSweepParams;
 typedef void (*GenSweepFn)(const GenSweepParams);
 struct GenSweepStream { int acc, xl, xr, yl, yr, zl, zr, rows, pz, slot_bytes, ns, off; };
 struct GenSweep {
-    GenSweepFn fn[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [fp64?][mode]; only the solution's element type is emitted
+    GenFnPair<GenSweepFn> fn[2][2];   // [fp64?][mode]; only the solution's element type is emitted
     int ty = 0, tz = 0, threads = 0, occ = 1, smem = 0;               // tile rows x z points, CTA size, CTAs per SM, dynamic smem
     std::vector<GenSweepStream> streams;
 };
@@ -74,7 +85,7 @@ struct GenPart {
     int fp_ops, reads, writes;
     std::vector<GenAccess> acc;
     std::vector<int> outs;           // indices into acc of the written accesses
-    GenKernelFn fn[2][2];            // [fp64?][mode: 0 strict, 1 fused]
+    GenKernelPair fn[2][2];          // [fp64?][mode: 0 strict, 1 fused]
     // Launch-box bounds derived from the part's sub-domain condition, per domain dim: global index range
     // [lo, hi] with each end = offset relative to 0 / first / last overall index (kind 0/1/2), kind -1 = open.
     struct Bound { int lo_kind, lo_off, hi_kind, hi_off; } bound[3];
@@ -94,7 +105,8 @@ struct GenStencil {
     std::vector<GenStage> stages;
 };
 
-#define GEN_FN(k, T, M) reinterpret_cast<yb::gen::GenKernelFn>(static_cast<void (*)(const yb::gen::GenParams)>(k<T, M>))
+#define GEN_FN1(k, T, M) reinterpret_cast<yb::gen::GenKernelFn>(static_cast<void (*)(const yb::gen::GenParams)>(k<T, M>))
+#define GEN_FN(k, T, M) yb::gen::GenKernelPair{GEN_FN1(k, T, M), GEN_FN1(k, T, (M) | yb::gen::GEN_WIDE)}
 
 #ifdef __CUDACC__
 // MODE 0: every operation individually rounded, in statement order (== the reference built with
@@ -119,10 +131,10 @@ template <> struct GenRn<double> {
 };
 template <typename T, int MODE> struct GenOp : GenRn<T> {
     using R = GenRn<T>;
-    static __device__ __forceinline__ T mad(T a, T b, T c) { return MODE == 0 ? R::add(R::mul(a, b), c) : R::fma(a, b, c); }
-    static __device__ __forceinline__ T msb(T a, T b, T c) { return MODE == 0 ? R::sub(R::mul(a, b), c) : R::fma(a, b, -c); }
-    static __device__ __forceinline__ T nmad(T a, T b, T c) { return MODE == 0 ? R::sub(c, R::mul(a, b)) : R::fma(-a, b, c); }
-    static __device__ __forceinline__ T nmsb(T a, T b, T c) { return MODE == 0 ? R::sub(-R::mul(a, b), c) : R::fma(-a, b, -c); }
+    static __device__ __forceinline__ T mad(T a, T b, T c) { return (MODE & 1) == 0 ? R::add(R::mul(a, b), c) : R::fma(a, b, c); }
+    static __device__ __forceinline__ T msb(T a, T b, T c) { return (MODE & 1) == 0 ? R::sub(R::mul(a, b), c) : R::fma(a, b, -c); }
+    static __device__ __forceinline__ T nmad(T a, T b, T c) { return (MODE & 1) == 0 ? R::sub(c, R::mul(a, b)) : R::fma(-a, b, c); }
+    static __device__ __forceinline__ T nmsb(T a, T b, T c) { return (MODE & 1) == 0 ? R::sub(-R::mul(a, b), c) : R::fma(-a, b, -c); }
 };
 
 // blockIdx.x -> (x, y, z) block coordinates in chunked sweep order (see GenParams::ychunk)
@@ -139,8 +151,15 @@ __device__ __forceinline__ void gen_block_coords(const GenParams& P, int& bx, in
     bz = int(rem % unsigned(P.nzb));
 }
 
+// Element position type of a direct kernel: int in the 32-bit form, long long in the 64-bit one (MODE & GEN_WIDE).
+template <int MODE> using GenIdx = typename std::conditional<(MODE & GEN_WIDE) != 0, long long, int>::type;
+template <int MODE>
+__device__ __forceinline__ GenIdx<MODE> gen_pos(const GenParams& P, int x, int y, int z) {
+    return GenIdx<MODE>(x) * P.SX + GenIdx<MODE>(y) * P.SY + z;
+}
+
 // One 128-byte line per thread and trip: lines of (GEN_BY * NP) rows x GEN_BZ points x GEN_BX planes per var.
-template <typename T>
+template <typename T, int MODE>
 __device__ __forceinline__ void gen_prefetch(const GenParams& P, int x0, int y0, int z0) {
     constexpr int LPR = GEN_BZ * int(sizeof(T)) / 128;              // lines per row
     constexpr int ROWS = GEN_BY * gen_np(int(sizeof(T))) * GEN_BX;
@@ -150,7 +169,7 @@ __device__ __forceinline__ void gen_prefetch(const GenParams& P, int x0, int y0,
         const int v = i / (ROWS * LPR), r = (i / LPR) % ROWS, l = i % LPR;
         const int xx = x0 + P.pfd + r / (GEN_BY * gen_np(int(sizeof(T)))), yy = y0 + r % (GEN_BY * gen_np(int(sizeof(T)))), zz = z0 + l * EPL;
         if (xx < P.xe && yy < P.ye && zz < P.ze) {
-            const T* a = static_cast<const T*>(P.ptr[P.pf[v]]) + (xx * P.SX + yy * P.SY + zz);
+            const T* a = static_cast<const T*>(P.ptr[P.pf[v]]) + gen_pos<MODE>(P, xx, yy, zz);
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
         }
     }
@@ -163,7 +182,7 @@ __device__ __forceinline__ void gen_prefetch(const GenParams& P, int x0, int y0,
     constexpr int GEN_NP = gen_np(int(sizeof(T)));                                               \
     const int y0_ = P.yb + gby_ * (GEN_BY * GEN_NP) + (threadIdx.x / GEN_BZ) % GEN_BY;           \
     const int x = P.xb + gbx_ * GEN_BX + threadIdx.x / (GEN_BZ * GEN_BY);                        \
-    if (P.npf) gen_prefetch<T>(P, P.xb + gbx_ * GEN_BX, P.yb + gby_ * (GEN_BY * GEN_NP), P.zb + gbz_ * GEN_BZ);       \
+    if (P.npf) gen_prefetch<T, MODE>(P, P.xb + gbx_ * GEN_BX, P.yb + gby_ * (GEN_BY * GEN_NP), P.zb + gbz_ * GEN_BZ);       \
     if (z >= P.ze || x >= P.xe) return;                                                          \
     _Pragma("unroll") for (int gp_ = 0; gp_ < GEN_NP; gp_++) {                                   \
         const int y = y0_ + gp_ * GEN_BY;                                                        \
@@ -172,7 +191,9 @@ __device__ __forceinline__ void gen_prefetch(const GenParams& P, int x0, int y0,
 // m = dim mask of the var (x=1, y=2, z=4).  Full-rank vars (m==7) use the shared geometry: one 64-bit position
 // per thread, 32-bit neighbour offsets that the compiler shares across vars; lower-rank vars (1-D sponge
 // arrays, scalars) take the general strided path.
-#define GEN_POS (x * P.SX + y * P.SY + z)   /* 32-bit: the engine refuses slots of 2^31 elements or more */
+// The position is 64-bit in the kernels' 64-bit form (slots of 2^31 elements or more; GenIdx); a neighbour offset stays 32-bit
+// because it is bounded by the halo times the plane stride, which the engine keeps below 2^31 (GenEngine::check_geometry).
+#define GEN_POS gen_pos<MODE>(P, x, y, z)
 #define RD(a, m, dx, dy, dz)                                                                                             \
     ((m) == 7 ? static_cast<const T*>(P.ptr[a])[GEN_POS + ((dx) * P.SX + (dy) * P.SY + (dz))]                              \
               : static_cast<const T*>(P.ptr[a])[(x + (dx)) * P.sx[a] + (y + (dy)) * P.sy[a] + (z + (dz)) * P.sz[a]])

@@ -34,7 +34,8 @@ struct GenSweepParams {
 // (GenSweepFn, GenSweepStream and GenSweep -- the host-side description filled in by the generated describe() -- are
 // declared in yb_gen.cuh next to GenPart.)
 
-#define GEN_SW_FN(k, M) reinterpret_cast<yb::gen::GenSweepFn>(static_cast<void (*)(const yb::gen::GenSweepParams)>(k<M>))
+#define GEN_SW_FN1(k, M) reinterpret_cast<yb::gen::GenSweepFn>(static_cast<void (*)(const yb::gen::GenSweepParams)>(k<M>))
+#define GEN_SW_FN(k, M) yb::gen::GenFnPair<yb::gen::GenSweepFn>{GEN_SW_FN1(k, M), GEN_SW_FN1(k, (M) | yb::gen::GEN_WIDE)}
 
 #ifdef __CUDACC__
 // The VW consecutive points of a thread: a 16-byte vector (float x 4, double x 2) or half of one (float x 2, double x 1).

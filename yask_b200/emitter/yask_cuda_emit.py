@@ -1058,7 +1058,7 @@ def emit_sweep_kernel(ir, p, plan, ident) -> list:
         L.append("                }")
     for o in p["outputs"]:
         a = o["access"]
-        L.append(f"                {{ T* dst = static_cast<T*>(P.ptr[{a}]) + (x * P.SX + y * P.SY + zq);")
+        L.append(f"                {{ T* dst = static_cast<T*>(P.ptr[{a}]) + gen_pos<MODE>(P, x, y, zq);")
         L.append(f"                  if (vec_ok) SwVec<T, VW>::stg(dst, o{a}); else for (int i = 0; i < nzv; i++) dst[i] = o{a}[i]; }}")
     L.append("            }")
     L.append("        }")
