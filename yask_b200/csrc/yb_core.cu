@@ -409,11 +409,19 @@ int yb_set_stream(yb_solution* s_, void* st) {
     return 0;
 }
 
+// Spare storage slots serve the temporal tile.  A rank grid drops them unless the engine keeps them for its fused rank-grid
+// mode (Engine::plan_storage), which also pads for the deeper halos of that mode.
+static void plan_storage(Solution& s) {
+    if (s.multi_rank()) for (auto& v : s.vars) if (!v.dev) v.extra_slots = 0;
+    s.engine->plan_storage(s);
+}
+
 int yb_solution_plan_geometry(yb_solution* s_) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
     if (s->prepared) return 0;
     if (int rc = compute_rank_geometry(*s)) return rc;
+    plan_storage(*s);
     for (auto& v : s->vars) compute_var_geometry(*s, v);
     return s->engine->check_geometry(*s);
 }
@@ -426,6 +434,7 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (ndev <= 0) return set_error(YB_ECUDA, "no CUDA device available: the yask_b200 engine has no CPU fallback");
     if (device < 0 || device >= ndev) return set_error(YB_EINVAL, "device %d out of range [0,%d)", device, ndev);
     if (int rc = compute_rank_geometry(*s)) return rc;
+    plan_storage(*s);
     // a size the kernels cannot address is refused before any storage is allocated
     for (auto& v : s->vars)
         if (!v.dev) compute_var_geometry(*s, v);
@@ -434,9 +443,6 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     s->device = device;
     if (!s->own_stream) YB_CUDA(cudaStreamCreateWithFlags(&s->own_stream, cudaStreamNonBlocking));
     if (!s->comm_stream) YB_CUDA(cudaStreamCreateWithFlags(&s->comm_stream, cudaStreamNonBlocking));
-    // extra storage slots serve the temporal tile, which runs on single-rank solutions only (the halo layer's peer
-    // addressing assumes the reference's slot count)
-    if (s->multi_rank()) for (auto& v : s->vars) if (!v.dev) v.extra_slots = 0;
     for (auto& v : s->vars) {
         const int64_t fvs = v.first_valid_step;
         const size_t had = v.dev ? v.bytes() : 0;
@@ -776,9 +782,10 @@ int yb_copy_to_host(void* host_dst, const void* dev_src, size_t bytes) {
 }
 
 // ---- run_solution ----------------------------------------------------------------------------------
-// Mirrors /root/reference/src/kernel/lib/context.cpp:220-624 for the no-wave-front case.  Single rank: one launch per
-// stage part over the whole rank box.  Multi-rank (halo_run_stage, yb_halo.cu): for each step, for each stage:
-// finish the previous exchange -> exterior slabs -> start this stage's exchange -> interior.
+// Mirrors /root/reference/src/kernel/lib/context.cpp:220-624.  Single rank: one launch per stage part over the whole rank box.
+// Multi-rank (halo_run_stage, yb_halo.cu): for each step, for each stage: finish the previous exchange -> exterior slabs ->
+// start this stage's exchange -> interior.  Multi-rank with fused steps (the reference's wave-fronts, -bt / -Mbt): one deep
+// exchange at the start, then per fused launch: finish the exchange -> whole rank box -> deep exchange (halo_run_steps).
 int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
@@ -816,12 +823,14 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     // direction from the order of the arguments, as the reference does (context.cpp:237-246)
     const int64_t step_dir = last_step >= first_step ? 1 : -1;
     if (rc >= 0) rc = s->engine->begin_run(*s, first_step, st);
-    // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward single-rank run goes through the engine's fused
-    // launch, `fs` steps at a time; what is left over (and every other kind of run) takes the one-step path below.
+    // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward run goes through the engine's fused launch, `fs` steps
+    // at a time; what is left over (and every other kind of run) takes the one-step path below.  A rank grid fuses steps only
+    // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.
     int64_t t_first = first_step;
-    const int fs = (step_dir > 0 && !s->halo && !s->tuner.enabled) ? s->engine->fused_steps(*s) : 1;
+    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled)) ? s->engine->fused_steps(*s) : 1;
+    if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
-        rc = s->engine->launch_steps(*s, t_first, fs, whole, st);
+        rc = s->halo ? halo_run_steps(*s, t_first, fs, st) : s->engine->launch_steps(*s, t_first, fs, whole, st);
         if (rc < 0) break;
         s->stats.kernel_launches += rc;
         for (int k = 0; k < fs; k++) {

@@ -132,6 +132,9 @@ struct Solution;
 // One implementation per stencil family: owns kernels, tensor maps and launch logic.
 struct Engine {
     virtual ~Engine() {}
+    // called by plan_geometry() and by prepare() once the rank geometry is known and before the vars' geometry is: storage that
+    // depends on the rank grid (spare slots, pads).  Default: nothing.
+    virtual void plan_storage(Solution&) {}
     // called by plan_geometry() and by prepare() once the vars' geometry is known and before any storage is allocated:
     // refuse a size the engine's kernels cannot address.  Default: no limit.
     virtual int check_geometry(const Solution&) const { return 0; }
@@ -155,6 +158,8 @@ struct Engine {
     virtual bool can_split(const Solution&, int /*stage*/) const { return true; }
     // Temporal tiling (the reference's block steps, "-bt"; /root/reference/src/kernel/lib/context.cpp:657-681): how many
     // consecutive steps one launch_steps() call may fuse for a forward run over the whole rank box (1 = no temporal tile).
+    // On a rank grid the answer is fixed at prepare, and halos are then exchanged once per fused launch (halo_run_steps):
+    // every rank of the grid must give the same one (yb_halo_import checks).
     virtual int fused_steps(const Solution&) const { return 1; }
     // called once per run_solution() before the first step (first_step = t of the first launch)
     virtual int begin_run(Solution&, int64_t /*first_step*/, cudaStream_t) { return 0; }

@@ -54,6 +54,7 @@ struct Blob {
     int64_t rank_size[3];
     cudaIpcMemHandle_t flags_handle;
     uint64_t flags_raw;
+    int32_t fused_steps;  // steps per halo exchange (Engine::fused_steps): neighbours must agree, or they would wait for each other's epochs
     BlobVar vars[MAX_VARS];
 };
 
@@ -243,7 +244,8 @@ static bool var_talks_to(const Var& v, const int dir[3]) {
     return true;
 }
 
-static int push_var_slot(Solution& s, const Neighbor& nb, int vi, int slot, cudaStream_t st) {
+// `depth` > 0: that many planes past the interface instead of the var's halo (fused rank-grid mode, halo_exchange_deep)
+static int push_var_slot(Solution& s, const Neighbor& nb, int vi, int slot, cudaStream_t st, int64_t depth = 0) {
     const Var& v = s.vars[vi];
     const BlobVar& pg = nb.var_geom[vi];
     int k4 = 0;
@@ -256,8 +258,8 @@ static int push_var_slot(Solution& s, const Neighbor& nb, int vi, int slot, cuda
         if (d.spec.kind == DIM_MISC) { first_src = 0; count = d.domain; first_dst = 0; }
         else {
             const int dk = nb.dir[d.spec.domain_index];
-            if (dk < 0) { count = d.spec.halo_r; first_src = 0; first_dst = pg.domain[k4]; }
-            else if (dk > 0) { count = d.spec.halo_l; first_src = d.domain - count; first_dst = -count; }
+            if (dk < 0) { count = depth > 0 ? depth : d.spec.halo_r; first_src = 0; first_dst = pg.domain[k4]; }
+            else if (dk > 0) { count = depth > 0 ? depth : d.spec.halo_l; first_src = d.domain - count; first_dst = -count; }
             else { count = d.domain; first_src = 0; first_dst = 0; }
             if (count > d.domain) return set_error(YB_EUNSUPPORTED, "rank domain smaller than halo in dim '%s'", d.spec.name.c_str());
             if (dk == 0 && pg.domain[k4] != d.domain) return set_error(YB_EINVAL, "neighbour has a different size in an unsplit dim");
@@ -383,6 +385,89 @@ int halo_exchange_all(Solution& s, cudaStream_t st) {
 }
 
 int halo_finish(Solution& s, cudaStream_t st) { return halo_flush_wait(s, st); }
+
+// Exchange of the fused rank-grid mode (the reference's wave-fronts: halos grow by the wave-front extension and are exchanged once
+// per fused launch, /root/reference/src/kernel/lib/setup.cpp:717-781).  A fused launch that computes steps t+1 and t+2 reads the
+// output var p(t) 2H and p(t-1) H deep past every rank interface (H = p's halo), and its inputs without a halo (v) H deep.  So:
+//   face neighbours: the slot of step t 2H deep, the slot of t-1 H deep and, with `with_inputs`, every input var without a halo
+//                    H deep (var_talks_to never sends those; they change only between runs);
+//   edge neighbours: the slot of step t H deep -- step 1 beyond one interface reads the points beyond the other (the reference
+//                    exchanges with every neighbour whenever it runs wave-fronts, alloc.cpp:504-510);
+//   anything else that is dirty, as halo_exchange_impl sends it.
+// Same epoch and WAR protocol as halo_exchange_impl, so every rank makes the same sequence of exchanges; the wait is left pending.
+int halo_exchange_deep(Solution& s, int64_t t, bool with_inputs, cudaStream_t st) {
+    HaloState* h = s.halo;
+    if (!h->finalized) return set_error(YB_ESTATE, "multi-rank solution: halo peers were not connected (yb_halo_import/finalize)");
+    if (int rc = halo_flush_wait(s, st)) return rc;
+    const StageSpec& sp = s.spec.stages[0];
+    const int pv = sp.outputs[0];
+    const Var& p = s.vars[pv];
+    int64_t H = 0;
+    for (auto& d : p.dims)
+        if (d.spec.kind == DIM_DOMAIN) H = std::max({H, d.spec.halo_l, d.spec.halo_r});
+    const int newest = p.slot_of(t), older = p.slot_of(t - 1);
+    auto haloless = [&](const Var& v) {
+        for (auto& d : v.dims)
+            if (d.spec.kind == DIM_DOMAIN && (d.spec.halo_l || d.spec.halo_r)) return false;
+        return v.domain_dim(0) && v.domain_dim(1) && v.domain_dim(2);
+    };
+    h->epoch++;
+    unsigned int mask = 0;
+    int launched = 0;
+    for (auto& nb : h->nbrs) {
+        const int l1 = abs(nb.dir[0]) + abs(nb.dir[1]) + abs(nb.dir[2]);
+        std::vector<std::pair<int, int>> sent;     // (var, slot) pushed deep to this neighbour
+        auto push = [&](int vi, int slot, int64_t depth) {
+            const int rc = push_var_slot(s, nb, vi, slot, st, depth);
+            if (rc >= 0) { launched += rc; sent.emplace_back(vi, slot); }
+            return rc;
+        };
+        int rc = 0;
+        if (l1 == 1) {
+            if (rc >= 0) rc = push(pv, newest, 2 * H);
+            if (rc >= 0) rc = push(pv, older, H);
+            if (with_inputs)
+                for (int vi : sp.inputs)
+                    if (rc >= 0 && vi != pv && haloless(s.vars[vi])) rc = push(vi, 0, H);
+        } else if (l1 == 2) {
+            rc = push(pv, newest, H);
+        }
+        for (size_t vi = 0; vi < s.vars.size() && rc >= 0; vi++) {
+            if (!var_talks_to(s.vars[vi], nb.dir)) continue;
+            for (int slot = 0; slot < s.vars[vi].nslots() && rc >= 0; slot++)
+                if (h->dirty[vi][slot] && std::find(sent.begin(), sent.end(), std::make_pair(int(vi), slot)) == sent.end()) rc = push(int(vi), slot, 0);
+        }
+        if (rc < 0) return rc;
+        int opp[3] = {-nb.dir[0], -nb.dir[1], -nb.dir[2]};
+        halo_signal_kernel<<<1, 1, 0, st>>>(nb.peer_flags + dir_index(opp), h->epoch);
+        mask |= 1u << dir_index(nb.dir);
+    }
+    YB_CUDA(cudaGetLastError());
+    h->wait_pending = true;
+    h->wait_mask = mask;
+    for (auto& dv : h->dirty)
+        for (auto& f : dv) f = 0;
+    s.stats.kernel_launches += launched;
+    return 0;
+}
+
+// `nsteps` steps from step t in ONE fused launch over the whole rank box (Engine::launch_steps), after the previous exchange has
+// arrived; then the deep exchange of the two newest steps.  Returns the number of kernels launched (the exchange's pushes are
+// counted by it).
+int halo_run_steps(Solution& s, int64_t t, int nsteps, cudaStream_t st) {
+    HaloState* h = s.halo;
+    if (!h->finalized) return set_error(YB_ESTATE, "multi-rank solution: halo peers were not connected (yb_halo_import/finalize)");
+    if (int rc = halo_flush_wait(s, st)) return rc;
+    Box whole;
+    for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = d < s.ndd ? s.rank_size[d] : 1; }
+    const int rc = s.engine->launch_steps(s, t, nsteps, whole, st);
+    if (rc < 0) return rc;
+    for (const StageSpec& sp : s.spec.stages)
+        for (int vi : sp.outputs)
+            for (int k = 1; k <= nsteps; k++) h->dirty[vi][s.vars[vi].slot_of(t + k)] = 1;
+    if (int e = halo_exchange_deep(s, t + nsteps, false, st)) return e;
+    return rc;
+}
 
 // Is anything but `var`'s slot `slot` waiting to be pushed?  (The in-kernel signal may only be used when the kernel's
 // own stores are the whole exchange.)
@@ -566,9 +651,10 @@ int yb_halo_export(yb_solution* s_, void* out, size_t nbytes) {
     YB_CUDA(cudaSetDevice(s->device));
     Blob b;
     memset(&b, 0, sizeof b);
-    b.magic = BLOB_MAGIC; b.version = 2; b.pid = int64_t(getpid()); b.nonce = process_nonce(); b.device = s->device;
+    b.magic = BLOB_MAGIC; b.version = 3; b.pid = int64_t(getpid()); b.nonce = process_nonce(); b.device = s->device;
     b.num_vars = int(s->vars.size());
     for (int k = 0; k < 3; k++) { b.rank_index[k] = s->rank_index[k]; b.rank_size[k] = s->rank_size[k]; }
+    b.fused_steps = s->engine->fused_steps(*s);
     YB_CUDA(cudaIpcGetMemHandle(&b.flags_handle, s->halo->flags));
     b.flags_raw = reinterpret_cast<uint64_t>(s->halo->flags);
     for (int i = 0; i < b.num_vars; i++) {
@@ -604,6 +690,11 @@ int yb_halo_import(yb_solution* s_, int64_t peer_rank_linear, const void* blob, 
         if (nb.peer_linear != peer_rank_linear) continue;
         for (int k = 0; k < 3; k++)
             if (b.rank_index[k] != s->rank_index[k] + nb.dir[k]) return set_error(YB_EINVAL, "blob of rank %lld has unexpected rank index", (long long)peer_rank_linear);
+        const int fs = s->engine->fused_steps(*s);
+        if (b.fused_steps != fs)
+            return set_error(YB_EINVAL, "rank %lld exchanges halos once per %d step(s) but its neighbour rank %lld once per %d: block_steps and "
+                                        "mega_block_steps must select the same mode on every rank", (long long)linear_rank(*s, s->rank_index), fs,
+                             (long long)peer_rank_linear, int(b.fused_steps));
         nb.same_process = (b.nonce == process_nonce());
         for (int i = 0; i < b.num_vars; i++) nb.var_geom[i] = b.vars[i];
         if (nb.same_process) {

@@ -295,6 +295,13 @@ struct IsoEngine : Engine {
     // temporal tile: option block_steps (the reference's -bt).  It needs two storage slots beyond the two the API sees
     // (Var::extra_slots), so it must be asked for before prepare_solution(); later changes only switch the launch path.
     int block_steps = 1;
+    // Rank grids (option mega_block_steps, the reference's -Mbt: halos are exchanged once per that many steps): with block_steps >= 2
+    // and mega_block_steps >= 2 set before prepare_solution() a rank grid keeps the spare slots, pads p 2R and v R deep on both sides
+    // of every split dim and runs the temporal tile on fused pairs, its halos exchanged once per pair (yb_halo.cu,
+    // halo_run_steps).  Decided in plan_storage(), i.e. at prepare: later changes of either option do not switch a rank grid's path.
+    int mega_block_steps = 1;
+    bool rank_pairs = false;
+    int64_t tt_launches = 0;       // read-only option tt_launches: fused launches since prepare
     bool tt_ok = false;            // extra slots allocated and tensor maps built
     TTMaps tt_maps[4];             // [slot of p(t)]; the variants of one radius share their box shapes
     int tt_variant = -1;           // option tt_variant: index into tt_radius_cfg(); -1 = the engine's choice (tt_var())
@@ -327,6 +334,7 @@ struct IsoEngine : Engine {
             if (t < -1 || t >= TT_VARIANTS) return YB_EINVAL;
             tt_variant = t;
         }
+        else if (k == "mega_block_steps") { mega_block_steps = std::max(1, atoi(v.c_str())); }
         else if (k == "block_steps") {
             block_steps = std::max(1, atoi(v.c_str()));
             if (!s.prepared && s.vars.size() >= 2) {
@@ -354,6 +362,8 @@ struct IsoEngine : Engine {
         else if (k == "lx") v = std::to_string(lx);
         else if (k == "grid") v = std::to_string(grid_override);
         else if (k == "block_steps") v = std::to_string(block_steps);
+        else if (k == "mega_block_steps") v = std::to_string(mega_block_steps);
+        else if (k == "tt_launches") v = std::to_string(tt_launches);
         else if (k == "tt_variant") v = std::to_string(tt_var());
         else return false;
         return true;
@@ -361,6 +371,37 @@ struct IsoEngine : Engine {
 
     // iso3dfd_sponge has no temporal tile: block_steps=2 runs one step per sweep, as in fp64
     static bool is_sponge(const StencilSpec& sp) { return sp.name == "iso3dfd_sponge"; }
+
+    // The fused rank-grid mode (rank_pairs): the spare slots of p that the core dropped on the rank grid, and pads on BOTH sides of
+    // every split dim -- the boxes of a fused launch reach p(t) 2R deep (z: the 8 elements of the boxes' 16-byte vectors) and
+    // p(t-1) / v R deep (z: 4) past a rank interface, where the halo exchange puts real data (on one rank, TMA zero-fills past the
+    // upper edge instead).
+    void plan_storage(Solution& s) override {
+        const int R = s.spec.radius;
+        rank_pairs = s.multi_rank() && block_steps >= 2 && mega_block_steps >= 2 && R <= TT_MAX_R && s.spec.elem_bytes == 4 &&
+                     !is_sponge(s.spec) && kernel != "direct" && s.vars.size() >= 2;
+        if (!rank_pairs || s.vars[0].dev) return;
+        s.vars[0].extra_slots = 2;
+        for (int vi = 0; vi < 2; vi++)
+            for (Dim& d : s.vars[vi].dims) {
+                if (d.spec.kind != DIM_DOMAIN) continue;
+                const int k = d.spec.domain_index;
+                const int64_t reach = vi == 0 ? (k == 2 ? 8 : 2 * R) : (k == 2 ? 4 : R);
+                d.min_pad_l = std::max<int64_t>(d.min_pad_l, reach);
+                if (s.num_ranks[k] > 1) d.min_pad_r = std::max<int64_t>(d.min_pad_r, reach);
+            }
+    }
+
+    // A rank of the fused mode computes its first step R points past each interface from halos 2R deep: the reference's minimum
+    // rank size with wave-fronts, halo + wave-front extension (/root/reference/src/kernel/lib/setup.cpp:760-772).
+    int check_geometry(const Solution& s) const override {
+        if (!rank_pairs) return 0;
+        for (int d = 0; d < s.ndd; d++)
+            if (s.num_ranks[d] > 1 && s.rank_size[d] < 2 * s.spec.radius)
+                return set_error(YB_EINVAL, "local-domain size of %lld in '%s' dim is less than minimum size of %d, which is based on stencil halos "
+                                            "and temporal wave-front sizes", (long long)s.rank_size[d], s.spec.domain_dims[d].c_str(), 2 * s.spec.radius);
+        return 0;
+    }
 
     int prepare(Solution& s) override {
         radius = s.spec.radius;
@@ -379,6 +420,7 @@ struct IsoEngine : Engine {
         num_sms = prop.multiProcessorCount;
         maps_ok = false;
         tt_ok = false;
+        tt_launches = 0;
         const int nsl = s.vars[0].nslots();
         if (nsl > 4) return set_error(YB_EUNSUPPORTED, "iso3dfd: at most 4 storage slots of p");
         if (prop.major >= 9 && f64) {
@@ -607,7 +649,8 @@ struct IsoEngine : Engine {
 
     // ---- temporal tile -------------------------------------------------------------------------------------------
     int fused_steps(const Solution& s) const override {
-        return (tt_ok && block_steps >= 2 && kernel != "direct" && !s.multi_rank()) ? 2 : 1;
+        if (s.multi_rank()) return (tt_ok && rank_pairs) ? 2 : 1;
+        return (tt_ok && block_steps >= 2 && kernel != "direct") ? 2 : 1;
     }
 
     // Halo cells of the spare pair of slots take those of the live pair, so that whichever pair a fused launch reads holds
@@ -660,6 +703,10 @@ struct IsoEngine : Engine {
         P.vel = reinterpret_cast<const float*>(v.slot_ptr(0)) + v.origin_offset();
         P.p_sx = px->stride; P.p_sy = py->stride; P.v_sx = vx->stride; P.v_sy = vy->stride;
         P.nx = int(px->domain); P.ny = int(py->domain); P.nz = int(pz->domain);
+        for (int k = 0; k < 3; k++) {       // step-1 points past a side with a neighbour rank are computed (fused rank-grid mode)
+            P.ext_lo[k] = s.rank_index[k] > 0 ? radius : 0;
+            P.ext_hi[k] = s.rank_index[k] < s.num_ranks[k] - 1 ? radius : 0;
+        }
         P.pad_x = int(px->pad_l); P.pad_y = int(py->pad_l); P.pad_z = int(pz->pad_l);
         P.vpad_x = int(vx->pad_l); P.vpad_y = int(vy->pad_l); P.vpad_z = int(vz->pad_l);
         for (int r = 0; r <= TT_MAX_R; r++) P.c[r] = r <= radius ? float(coef[r]) : 0.f;
@@ -696,6 +743,7 @@ struct IsoEngine : Engine {
         }
         c.fn[mode]<<<grid, c.threads, c.smem, st>>>(tt_maps[cur], P);
         YB_CUDA(cudaGetLastError());
+        tt_launches++;
         p.slot_bias ^= 2;       // steps t+1, t+2 (and every later access, stream-ordered) live in the other pair now
         return 1;
     }

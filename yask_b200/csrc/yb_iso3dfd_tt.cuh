@@ -12,8 +12,10 @@
 //             p(t-1), v  plane x1 = xl - R  over the tile + R rows / HZ1 columns        -> rings of PF+1 planes
 //             (three TMA 3-D boxes, cp.async.bulk.tensor; completion on full[g mod (PF+1)])
 //   step 1  : p(t+1) at plane x1 over the tile + R ring, from the p(t) ring -> p1 ring (shared memory, 2R+2 planes);
-//             the tile's own part also goes to HBM (slot of t+1).  Points outside the domain take p(t-1): the value
+//             the tile's own part also goes to HBM (slot of t+1).  Points outside the global domain take p(t-1): the value
 //             the reference's two-slot storage holds in the halo cells of p(t+1) (/root/reference/src/compiler/lib/Var.cpp:435-464).
+//             Points in the R ring beyond a rank interface are computed like any other (TTParams::ext_lo / ext_hi): the
+//             reference's wave-front extension of a rank, whose halos are exchanged once per pair of steps.
 //   barrier : __syncthreads (the only one per iteration); then thread 0 issues the loads of iteration g+PF
 //   step 2  : p(t+2) at plane x2 = x1 - R over the tile, from the p1 ring (x2-R..x2+R), p(t) plane x2 (the oldest plane of
 //             the p ring, "prev") and v(x2) (read from global/L2 into a register before step 1) -> HBM (slot of t+2).
@@ -56,7 +58,12 @@ struct TTParams {
     const float* vel;          // &v[domain origin]
     long long p_sx, p_sy;      // element strides of the p slots (z stride 1)
     long long v_sx, v_sy;
-    int nx, ny, nz;            // rank-domain sizes (the temporal tile runs on whole single-rank domains)
+    int nx, ny, nz;            // rank-domain sizes (the temporal tile runs on whole rank domains)
+    // Step-1 points with -ext_lo[d] <= index < n[d] + ext_hi[d] in every dim (x, y, z) are computed; the others lie outside the
+    // GLOBAL domain and take p(t-1).  0 on a side at the global boundary (so a zero-initialised TTParams describes one rank); R on a
+    // side with a neighbour rank, whose halos hold p(t) 2R deep and p(t-1), v R deep, so that the step-1 ring there is what the
+    // neighbour computes for its own points.
+    int ext_lo[3], ext_hi[3];
     int pad_x, pad_y, pad_z;   // p: alloc index of the domain origin (TMA coordinates)
     int vpad_x, vpad_y, vpad_z;
     int nty, ntz, nchunks;     // tiles in y and z, chunks along x
@@ -234,8 +241,8 @@ YB_DEVFN void tt_thread_setup(TTThread<T>& th, const TTParams& P, const TTCursor
             th.io1[k] = (row + R) * T::IZ + T::HZ1 + 4 * q;   // p(t) planes start at row y0-2R, column z0-2*HZ1
             th.so1[k] = row * T::S1Z + 4 * q;                 // step-1 planes start at row y0-R, column z0-HZ1
             int m = 0;
-            if (gy >= 0 && gy < P.ny)
-                for (int i = 0; i < 4; i++) if (gz + i >= 0 && gz + i < P.nz) m |= 1 << i;
+            if (gy >= -P.ext_lo[1] && gy < P.ny + P.ext_hi[1])
+                for (int i = 0; i < 4; i++) if (gz + i >= -P.ext_lo[2] && gz + i < P.nz + P.ext_hi[2]) m |= 1 << i;
             th.in1[k] = m;
             const bool centre = row >= R && row < R + T::TY && q >= T::ZQ && q < T::ZQ + T::S2Q;
             if (centre && gy < P.ny && gz < P.nz) {
@@ -338,7 +345,7 @@ YB_DEVFN void tt_step1(uint8_t* sm, const TTParams& P, const TTCursor& cu, const
     const float* prevp = reinterpret_cast<const float*>(sm + T::PV_OFF + rg.gs * T::S_SLOT);
     const float* vp = reinterpret_cast<const float*>(sm + T::V_OFF + rg.gs * T::S_SLOT);
     float* p1 = reinterpret_cast<float*>(sm + T::P1_OFF + rg.g1 * T::S_SLOT);
-    const bool x_in = x1 >= 0 && x1 < P.nx;
+    const bool x_in = x1 >= -P.ext_lo[0] && x1 < P.nx + P.ext_hi[0];
     const bool x_store = x1 >= cu.cx0 && x1 < cu.cx0 + cu.len;
     float* o1 = P.out1 + (long long)x1 * P.p_sx;
 #pragma unroll
@@ -431,7 +438,7 @@ YB_DEVFN void tt_step1_xq(uint8_t* sm, const TTParams& P, const TTCursor& cu, TT
     const float* prevp = reinterpret_cast<const float*>(sm + T::PV_OFF + rg.gs * T::S_SLOT);
     const float* vp = reinterpret_cast<const float*>(sm + T::V_OFF + rg.gs * T::S_SLOT);
     float* p1 = reinterpret_cast<float*>(sm + T::P1_OFF + rg.g1 * T::S_SLOT);
-    const bool x_in = x1 >= 0 && x1 < P.nx;
+    const bool x_in = x1 >= -P.ext_lo[0] && x1 < P.nx + P.ext_hi[0];
     const bool x_store = x1 >= cu.cx0 && x1 < cu.cx0 + cu.len;
     float* o1 = P.out1 + (long long)x1 * P.p_sx;
 #pragma unroll

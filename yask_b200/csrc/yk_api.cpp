@@ -545,6 +545,8 @@ struct B200Solution : yk_solution {
         else (void)yb_set_option(h->s, "block_steps", std::to_string(size < 1 ? 1 : size).c_str());    // engines without one refuse: fine
         block_size[dim] = size;
     }
+    // Mega-block steps of the step dim (the reference's -Mbt): engines without a fused rank-grid mode refuse the option: fine.
+    void set_mega_block_steps(idx_t n) { (void)yb_set_option(h->s, "mega_block_steps", std::to_string(n < 1 ? 1 : n).c_str()); }
     void set_block_size_vec(const idx_t_vec& v) override { auto d = get_domain_dim_names(); if (v.size() != d.size()) fail("set_block_size_vec: wrong number of values"); for (size_t k = 0; k < d.size(); k++) block_size[d[k]] = v[k]; }
     void set_block_size_vec(const idx_t_init_list& v) override { set_block_size_vec(idx_t_vec(v)); }
     idx_t get_block_size(const std::string& dim) const override {
@@ -576,7 +578,7 @@ struct B200Solution : yk_solution {
                                              "force_scalar_exchange", "bundle_allocs", "bind_inner_threads", "allow_addl_padding", "use_device_mpi",
                                              "print_suffixes", "trace", "validate", "find_loc"};
         static const char* ignored_val[] = {"outer_threads", "inner_threads", "max_threads", "thread_divisor", "numa_pref", "msg_rank", "min_exterior",
-                                            "auto_tune_trial_secs", "auto_tune_radius", "auto_tune_targets", "Mbt", "mbt", "ep", "mp_extra"};
+                                            "auto_tune_trial_secs", "auto_tune_radius", "auto_tune_targets", "mbt", "ep", "mp_extra"};
         for (size_t a = 0; a < args.size(); a++) {
             const std::string& arg = args[a];
             bool used = false;
@@ -587,6 +589,9 @@ struct B200Solution : yk_solution {
                 if (key == "auto_tune" || key == "no-auto_tune") { chk(yb_solution_reset_auto_tuner(h->s, key[0] == 'n' ? 0 : 1)); used = true; }
                 if (key == "overlap_comms" || key == "no-overlap_comms") { chk(yb_set_option(h->s, "overlap_comms", key[0] == 'n' ? "0" : "1")); used = true; }
                 if (key == "bt") { set_block_size(get_step_dim_name(), atoll(take().c_str())); used = true; }     // temporal tile
+                // the reference's mega-block steps (wave-front steps): on a rank grid, halos are exchanged once per that many steps.
+                // Unlike the reference it does not default to -bt (there -bt alone keeps one exchange per step on a rank grid).
+                if (key == "Mbt") { set_mega_block_steps(atoll(take().c_str())); used = true; }
                 if (!used) for (auto* b : ignored_bool) if (key == b || key == std::string("no-") + b) used = true;
                 if (!used) for (auto* v : ignored_val) if (key == v) { take(); used = true; }
                 if (!used) {
@@ -630,6 +635,7 @@ struct B200Solution : yk_solution {
                " -nr<dim> <n>  ranks in dim               -ri<dim> <n>  rank index in dim\n"
                " -mp<dim> <n>  minimum padding            -b<dim> <n>   block size (recorded; no effect on the GPU)\n"
                " -bt <n>       block steps: n >= 2 selects the temporal tile where the engine has one (iso3dfd radius <= 2)\n"
+               " -Mbt <n>      mega-block steps: with -bt 2, n >= 2 runs the temporal tile on rank grids too, halos exchanged once per 2 steps\n"
                " -fp_mode 0|1|2  FP contraction mode      -kernel auto|tma|direct   -tile <n>   -lx <n>   -device <n>\n";
     }
     std::string get_command_line_values() override {
@@ -638,6 +644,8 @@ struct B200Solution : yk_solution {
         for (size_t k = 0; k < d.size(); k++)
             os << " -g" << d[k] << " " << yb_get_overall_domain_size(h->s, int(k)) << " -l" << d[k] << " " << yb_get_rank_domain_size(h->s, int(k)) << " -nr" << d[k]
                << " " << yb_get_num_ranks(h->s, int(k)) << " -ri" << d[k] << " " << yb_get_rank_index(h->s, int(k));
+        char mbt[32];
+        if (yb_get_option(h->s, "mega_block_steps", mbt, sizeof mbt) == 0) os << " -Mbt " << mbt;
         return os.str();
     }
     int get_num_vars() const override { return yb_num_vars(h->s); }

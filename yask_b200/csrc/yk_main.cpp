@@ -59,6 +59,7 @@ int main(int argc, char** argv) {
         double init_val = 0.1, init_seed = 0.1;
         bool pre_auto_tune = true;
         bool validate = false;
+        idx_t mega_block_steps = 0;      // -Mbt: steps per halo exchange of a rank grid's temporal tile (reported as num-wave-front-steps)
         // harness options first; everything else goes to the solution (as yask_main.cpp:199-259 does)
         string_vec rest;
         for (int i = 1; i < argc; i++) {
@@ -79,6 +80,7 @@ int main(int argc, char** argv) {
             else if (a == "-validate" || a == "-v") validate = true;
             else if (a == "-pre_auto_tune") pre_auto_tune = true;          // yask_main.cpp:53: on by default
             else if (a == "-no-pre_auto_tune") pre_auto_tune = false;
+            else if (a == "-Mbt") { rest.push_back(a); rest.push_back(val()); mega_block_steps = atoll(rest.back().c_str()); }   // also the solution's
             else rest.push_back(a);
         }
         // only one rank of a job prints (yask_main.cpp -msg_rank)
@@ -119,7 +121,8 @@ int main(int argc, char** argv) {
             << " stencil-name:           " << soln->get_name() << "\n"
             << " stencil-description:    " << soln->get_description() << "\n"
             << " element-size:           " << soln->get_element_bytes() << "B\n"
-            << " num-temporal-block-steps:  " << std::max<idx_t>(1, soln->get_block_size(soln->get_step_dim_name())) << "\n";
+            << " num-temporal-block-steps:  " << std::max<idx_t>(1, soln->get_block_size(soln->get_step_dim_name())) << "\n"
+            << " num-wave-front-steps:      " << std::max<idx_t>(1, mega_block_steps) << "\n";
 
         // data: every var constant, slightly different per var (the reference's init_same pattern)
         int k = 0;
