@@ -8,6 +8,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include "yb_chunk_plan.h"
 #include "yb_core.h"
 #include "yb_iso3dfd.cuh"
 #include "yb_iso3dfd_tiles.h"
@@ -148,27 +149,9 @@ EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// 3-D tiled map over one step slot of a var (dims x,y,z; z unit stride) with box (bz, by, 1); FLOAT32 or FLOAT64 elements.
-int make_map(CUtensorMap* map, const Var& v, int slot, int bz, int by) {
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) return set_error(YB_ECUDA, "cuTensorMapEncodeTiled not available from the driver");
-    const Dim* dx = v.domain_dim(0);
-    const Dim* dy = v.domain_dim(1);
-    const Dim* dz = v.domain_dim(2);
-    cuuint64_t gdim[3] = {cuuint64_t(dz->alloc), cuuint64_t(dy->alloc), cuuint64_t(dx->alloc)};
-    const cuuint64_t eb = cuuint64_t(v.elem_bytes);
-    cuuint64_t gstr[2] = {cuuint64_t(dy->stride) * eb, cuuint64_t(dx->stride) * eb};
-    cuuint32_t box[3] = {cuuint32_t(bz), cuuint32_t(by), 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(map, v.elem_bytes == 8 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT64 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, v.slot_ptr(slot), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(YB_ECUDA, "cuTensorMapEncodeTiled failed with code %d", int(r));
-    return 0;
-}
-
 }  // namespace
 
-// 3-D tiled map over one step slot of a full-rank var of any element size (generated sweep kernels, yb_gen.cu).
+// 3-D tiled map over one step slot of a full-rank var of any element size (iso3dfd sweeps; generated sweep kernels, yb_gen.cu).
 int make_var_tensor_map(void* map_, const Var& v, int slot, int box_z, int box_y) {
     CUtensorMap* map = static_cast<CUtensorMap*>(map_);
     EncodeTiledFn enc = get_encode_fn();
@@ -191,36 +174,29 @@ int make_var_tensor_map(void* map_, const Var& v, int slot, int box_z, int box_y
 
 namespace {
 
-template <class T, int PW, int U>
-TileCfg cfg_tile(const char* name) {
-    return TileCfg{true, name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128 * PW, T::SMEM_BYTES,
-                   {iso3dfd_tma2_kernel<T, 0, PW, U>, iso3dfd_tma2_kernel<T, 1, PW, U>, iso3dfd_tma2_kernel<T, 2, PW, U>,
-                    iso3dfd_tma2_kernel<T, 3, PW, U>}};
-}
-
 // Compiled variants of the sweep kernel for radius 8 (option `tile`): tile shape x producer warpgroup x planes per trip.
 constexpr int NTILES = 8;
 constexpr int DEFAULT_TILE = 7;
 const TileCfg& tile_cfg(int i) {
     static const TileCfg cfgs[NTILES] = {
-        cfg_tile<IsoTile2<8, 16, 16, 5>, 0, 1>("32x64, in-loop producer"),
-        cfg_tile<IsoTile2<8, 8, 32, 5>, 0, 1>("16x128, in-loop producer"),
-        cfg_tile<IsoTile2<8, 16, 16, 5>, 1, 1>("32x64 + producer warpgroup"),
-        cfg_tile<IsoTile2<8, 16, 16, 5>, 0, 2>("32x64, 2 planes per trip"),
-        cfg_tile<IsoTile2<8, 8, 32, 5>, 1, 1>("16x128 + producer warpgroup"),
-        cfg_tile<IsoTile2<8, 8, 32, 5>, 0, 2>("16x128, 2 planes per trip"),
-        cfg_tile<IsoTile2<8, 16, 16, 5>, 1, 2>("32x64 + producer warpgroup, 2 planes per trip"),
-        cfg_tile<IsoTile2<8, 8, 32, 5>, 1, 2>("16x128 + producer warpgroup, 2 planes per trip"),
+        iso_tile_cfg<IsoTile2<8, 16, 16, 5>, 0, 1, true>("32x64, in-loop producer"),
+        iso_tile_cfg<IsoTile2<8, 8, 32, 5>, 0, 1, true>("16x128, in-loop producer"),
+        iso_tile_cfg<IsoTile2<8, 16, 16, 5>, 1, 1, true>("32x64 + producer warpgroup"),
+        iso_tile_cfg<IsoTile2<8, 16, 16, 5>, 0, 2, true>("32x64, 2 planes per trip"),
+        iso_tile_cfg<IsoTile2<8, 8, 32, 5>, 1, 1, true>("16x128 + producer warpgroup"),
+        iso_tile_cfg<IsoTile2<8, 8, 32, 5>, 0, 2, true>("16x128, 2 planes per trip"),
+        iso_tile_cfg<IsoTile2<8, 16, 16, 5>, 1, 2, true>("32x64 + producer warpgroup, 2 planes per trip"),
+        iso_tile_cfg<IsoTile2<8, 8, 32, 5>, 1, 2, true>("16x128 + producer warpgroup, 2 planes per trip"),
     };
     return cfgs[i];
 }
 
 // Resident-plane form (option `resident`, iso3dfd_tma3_kernel) of the radius-8 producer-warpgroup, 2-planes-per-trip variants:
-// same tile shapes, so it shares their tensor maps.  Rings within the 227 KB opt-in: 16x128 (18 KB slots) 10 slots = 1 plane of
-// prefetch; 32x64 (15 KB slots) 12 slots = 3 planes; both with 2 stages of p(t-1) / v.  nullptr for the other tiles.
+// same tile shapes as tiles 6 and 7.  Rings within the 227 KB opt-in: 16x128 (18 KB slots) 10 slots = 1 plane of prefetch; 32x64
+// (15 KB slots) 12 slots = 3 planes; both with 2 stages of p(t-1) / v.  nullptr for the other tiles.
 template <class T>
 TileCfg cfg_resident(const char* name) {
-    return TileCfg{true, name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128, T::SMEM_BYTES,
+    return TileCfg{name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128, T::SMEM_BYTES,
                    {iso3dfd_tma3_kernel<T, 0>, iso3dfd_tma3_kernel<T, 1>, iso3dfd_tma3_kernel<T, 2>, iso3dfd_tma3_kernel<T, 3>}};
 }
 const TileCfg* resident_cfg(int tile) {
@@ -258,6 +234,42 @@ const TTCfg* tt_radius_cfg(int radius, int variant) {
     return (radius >= 1 && radius <= TT_MAX_R && variant >= 0 && variant < TT_VARIANTS) ? &cfgs[radius - 1][variant] : nullptr;
 }
 
+// One launchable form of a sweep kernel: its table entry, its tensor maps for every slot of p(t), and per FP mode whether the
+// kernel's dynamic shared-memory size is set.  That is done at the mode's first launch, since setting it loads the kernel.
+template <class Cfg, class Maps>
+struct SweepForm {
+    const Cfg* cfg;
+    Maps maps[4];               // [slot of p(t)]; p(t-1) is its partner (slot ^ 1) in the live pair of slots
+    bool attr_set[4] = {};
+    template <class Params>
+    int launch(int mode, int cur, int grid, const Params& P, cudaStream_t st) {
+        if (!attr_set[mode]) {
+            YB_CUDA(cudaFuncSetAttribute(cfg->fn[mode], cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg->smem)));
+            attr_set[mode] = true;
+        }
+        cfg->fn[mode]<<<grid, cfg->threads, cfg->smem, st>>>(maps[cur], P);
+        return 0;
+    }
+};
+// A form of the one-step sweep, with the option values that select it: tile (-1: the one form of its radius and precision) and
+// the resident-plane form.
+template <class E>
+struct IsoSweep : SweepForm<TileCfgT<E>, IsoMaps> {
+    int tile;
+    bool resident;
+};
+
+// The reference-order direct kernel by [sponge][FP mode]: thin slabs, kernel=direct and the on-device cross-check.
+template <class E>
+using DirectFn = void (*)(IsoParamsT<E>, int);
+template <class E>
+DirectFn<E> direct_kernel(bool sponge, int mode) {
+    static const DirectFn<E> fns[2][3] = {
+        {iso3dfd_direct_kernel<E, 0>, iso3dfd_direct_kernel<E, 1>, iso3dfd_direct_kernel<E, 2>},
+        {iso3dfd_direct_kernel<E, 0, true>, iso3dfd_direct_kernel<E, 1, true>, iso3dfd_direct_kernel<E, 2, true>}};
+    return fns[sponge][mode];
+}
+
 // Copies a box of cells from one step slot to another (same geometry): keeps the halo cells of the extra storage
 // slots of a temporally tiled var equal to those of the slot two steps earlier -- what the reference's two-slot storage
 // gives by construction (p(t+2) lives in the memory of p(t), halo cells included).
@@ -283,14 +295,14 @@ struct IsoEngine : Engine {
     int lx = 0;                    // planes per sweep chunk (0 = choose per launch)
     int grid_override = 0;
     int num_sms = 148;
-    bool attr_set[NTILES + 2][4] = {};    // [cfg_index()][FP mode]
     // L2 policy of the sweep: both p(t) streams evict_last (a plane is fetched halo-less 8 sweep steps before it is fetched
     // with its halo, and its halo rows are the neighbouring tiles' centre rows), p(t-1) / v evict_first (streamed once), results
     // leave with streaming stores
     int pol_c = 2, pol_h = 2, pol_pv = 1, st_cs = 1;
     bool mem_probe = false;      // debug: fp_mode=3 style memory-only kernel
     int peer_probe = 0;          // debug: see IsoParams::peer_probe
-    IsoMaps maps[NTILES][4];       // [tile][slot of p(t)]; p(t-1) is its partner (slot ^ 1) in the live pair of slots
+    std::vector<IsoSweep<float>> sweeps_f32;      // the one-step sweep forms built at prepare (sweep())
+    std::vector<IsoSweep<double>> sweeps_f64;
     bool maps_ok = false;
     // temporal tile: option block_steps (the reference's -bt).  It needs two storage slots beyond the two the API sees
     // (Var::extra_slots), so it must be asked for before prepare_solution(); later changes only switch the launch path.
@@ -303,13 +315,12 @@ struct IsoEngine : Engine {
     bool rank_pairs = false;
     int64_t tt_launches = 0;       // read-only option tt_launches: fused launches since prepare
     bool tt_ok = false;            // extra slots allocated and tensor maps built
-    TTMaps tt_maps[4];             // [slot of p(t)]; the variants of one radius share their box shapes
+    std::vector<SweepForm<TTCfg, TTMaps>> tts;    // [tt_var()]
     int tt_variant = -1;           // option tt_variant: index into tt_radius_cfg(); -1 = the engine's choice (tt_var())
     // The shared-memory form at both radii.  Radius 2, 1024^3, H100 80GB HBM3: 5.53-5.59 against 6.10 ms/step for the register-queue
     // form in three interleaved runs of each at a 700 W power limit (5.66 against 6.37 in one run at 400 W); radius 1: within 3 % of
     // the fastest form in one run
     int tt_var() const { return tt_variant >= 0 ? tt_variant : 0; }
-    bool tt_attr_set[TT_VARIANTS][3] = {};
 
     int set_option(Solution& s, const std::string& k, const std::string& v) override {
         if (k == "kernel") {
@@ -338,18 +349,8 @@ struct IsoEngine : Engine {
         else if (k == "block_steps") {
             block_steps = std::max(1, atoi(v.c_str()));
             if (!s.prepared && s.vars.size() >= 2) {
-                const bool on = block_steps >= 2 && s.spec.radius <= TT_MAX_R && s.spec.elem_bytes == 4 && !is_sponge(s.spec);
-                s.vars[0].extra_slots = on ? 2 : 0;
-                if (on) {
-                    // the tile's boxes reach 2R rows / planes (p) and R rows / planes, one 16-byte vector in z (v) below the
-                    // domain origin: pad that far, so that no TMA coordinate is ever negative (boxes that stick out at the
-                    // upper end are zero-filled by the hardware, as in the one-step kernels on ragged domains)
-                    const int R = s.spec.radius;
-                    for (Dim& d : s.vars[0].dims)
-                        if (d.spec.kind == DIM_DOMAIN) d.min_pad_l = std::max<int64_t>(d.min_pad_l, d.spec.domain_index == 2 ? 8 : 2 * R);
-                    for (Dim& d : s.vars[1].dims)
-                        if (d.spec.kind == DIM_DOMAIN) d.min_pad_l = std::max<int64_t>(d.min_pad_l, d.spec.domain_index == 2 ? 4 : R);
-                }
+                s.vars[0].extra_slots = 0;
+                if (block_steps >= 2 && tt_capable(s.spec)) add_tt_storage(s, false);
             }
         }
         else return YB_EINVAL;
@@ -371,16 +372,16 @@ struct IsoEngine : Engine {
 
     // iso3dfd_sponge has no temporal tile: block_steps=2 runs one step per sweep, as in fp64
     static bool is_sponge(const StencilSpec& sp) { return sp.name == "iso3dfd_sponge"; }
+    // The temporal tile computes plain iso3dfd in fp32 at radius 1..TT_MAX_R.
+    static bool tt_capable(const StencilSpec& sp) { return sp.radius <= TT_MAX_R && sp.elem_bytes == 4 && !is_sponge(sp); }
 
-    // The fused rank-grid mode (rank_pairs): the spare slots of p that the core dropped on the rank grid, and pads on BOTH sides of
-    // every split dim -- the boxes of a fused launch reach p(t) 2R deep (z: the 8 elements of the boxes' 16-byte vectors) and
-    // p(t-1) / v R deep (z: 4) past a rank interface, where the halo exchange puts real data (on one rank, TMA zero-fills past the
-    // upper edge instead).
-    void plan_storage(Solution& s) override {
+    // The temporal tile's storage: the spare pair of slots of p, and pads as deep as its boxes reach past the domain -- p(t) 2R
+    // rows / planes (z: the 8 elements of the boxes' 16-byte vectors), p(t-1) and v R (z: 4) -- so that no TMA coordinate is ever
+    // negative.  Below the origin always; with split_sides also above it in every dim split over ranks, where the halo exchange of
+    // the fused rank-grid mode puts real data (on one rank, boxes that stick out at the upper end are zero-filled by the hardware,
+    // as in the one-step kernels on ragged domains).
+    static void add_tt_storage(Solution& s, bool split_sides) {
         const int R = s.spec.radius;
-        rank_pairs = s.multi_rank() && block_steps >= 2 && mega_block_steps >= 2 && R <= TT_MAX_R && s.spec.elem_bytes == 4 &&
-                     !is_sponge(s.spec) && kernel != "direct" && s.vars.size() >= 2;
-        if (!rank_pairs || s.vars[0].dev) return;
         s.vars[0].extra_slots = 2;
         for (int vi = 0; vi < 2; vi++)
             for (Dim& d : s.vars[vi].dims) {
@@ -388,8 +389,16 @@ struct IsoEngine : Engine {
                 const int k = d.spec.domain_index;
                 const int64_t reach = vi == 0 ? (k == 2 ? 8 : 2 * R) : (k == 2 ? 4 : R);
                 d.min_pad_l = std::max<int64_t>(d.min_pad_l, reach);
-                if (s.num_ranks[k] > 1) d.min_pad_r = std::max<int64_t>(d.min_pad_r, reach);
+                if (split_sides && s.num_ranks[k] > 1) d.min_pad_r = std::max<int64_t>(d.min_pad_r, reach);
             }
+    }
+
+    // The fused rank-grid mode (rank_pairs): the spare slots of p that the core dropped on the rank grid, padded on both sides of
+    // every split dim.
+    void plan_storage(Solution& s) override {
+        rank_pairs = s.multi_rank() && block_steps >= 2 && mega_block_steps >= 2 && tt_capable(s.spec) && kernel != "direct" &&
+                     s.vars.size() >= 2;
+        if (rank_pairs && !s.vars[0].dev) add_tt_storage(s, true);
     }
 
     // A rank of the fused mode computes its first step R points past each interface from halos 2R deep: the reference's minimum
@@ -421,79 +430,80 @@ struct IsoEngine : Engine {
         maps_ok = false;
         tt_ok = false;
         tt_launches = 0;
+        sweeps_f32.clear();
+        sweeps_f64.clear();
+        tts.clear();
         const int nsl = s.vars[0].nslots();
         if (nsl > 4) return set_error(YB_EUNSUPPORTED, "iso3dfd: at most 4 storage slots of p");
-        if (prop.major >= 9 && f64) {
-            const TileCfgT<double>& c = sweep_cfg<double>();
-            for (int cur = 0; cur < nsl; cur++)
-                if (int rc = make_maps(s, c, cur, maps[0][cur])) return rc;
+        if (prop.major >= 9) {
+            if (int rc = f64 ? build_sweeps<double>(s, nsl) : build_sweeps<float>(s, nsl)) return rc;
             maps_ok = true;
-            for (int m = 0; m < 3; m++) preload_kernel((const void*)c.fn[m]);
-        } else if (prop.major >= 9 && (radius == 8 || iso_radius_cfg(radius))) {
-            const Var& p = s.vars[0];
-            const Var& v = s.vars[1];
-            for (int tl = 0; tl < (radius == 8 ? NTILES : 1); tl++) {
-                const TileCfg& c = radius == 8 ? tile_cfg(tl) : sweep_cfg<float>();
-                for (int cur = 0; cur < nsl; cur++)
-                    if (int rc = make_maps(s, c, cur, maps[tl][cur])) return rc;
-            }
-            maps_ok = true;
-            // (the temporal tile computes plain iso3dfd: never for a sponge solution, whatever gave p its spare slots)
-            if (const TTCfg* tc = (p.extra_slots == 2 && nsl == 4 && !sponge) ? tt_radius_cfg(radius, 0) : nullptr) {
-                for (int cur = 0; cur < nsl; cur++) {
-                    TTMaps& m = tt_maps[cur];
-                    if (int rc = make_map(&m.pin, p, cur, tc->iz, tc->iy)) return rc;
-                    if (int rc = make_map(&m.prev, p, cur ^ 1, tc->s1z, tc->s1y)) return rc;
-                    if (int rc = make_map(&m.v, v, 0, tc->s1z, tc->s1y)) return rc;
+            if (tt_capable(s.spec) && s.vars[0].extra_slots == 2 && nsl == 4) {
+                const Var& p = s.vars[0];
+                const Var& v = s.vars[1];
+                for (int vr = 0; vr < TT_VARIANTS; vr++) {
+                    SweepForm<TTCfg, TTMaps> w{tt_radius_cfg(radius, vr)};
+                    for (int cur = 0; cur < nsl; cur++) {
+                        TTMaps& m = w.maps[cur];
+                        if (int rc = make_var_tensor_map(&m.pin, p, cur, w.cfg->iz, w.cfg->iy)) return rc;
+                        if (int rc = make_var_tensor_map(&m.prev, p, cur ^ 1, w.cfg->s1z, w.cfg->s1y)) return rc;
+                        if (int rc = make_var_tensor_map(&m.v, v, 0, w.cfg->s1z, w.cfg->s1y)) return rc;
+                    }
+                    for (int m = 0; m < 3; m++) preload_kernel((const void*)w.cfg->fn[m]);
+                    tts.push_back(w);
                 }
                 tt_ok = true;
-                for (int vr = 0; vr < TT_VARIANTS; vr++)
-                    for (int m = 0; m < 3; m++) preload_kernel((const void*)tt_radius_cfg(radius, vr)->fn[m]);
                 preload_kernel((const void*)slot_box_copy_kernel);
             }
-            const TileCfg& c = sweep_cfg<float>();
-            for (int m = 0; m < 4; m++) preload_kernel((const void*)c.fn[m]);
         }
-        if (sponge) {
-            const void* fns[2][3] = {{(const void*)iso3dfd_direct_kernel<float, 0, true>, (const void*)iso3dfd_direct_kernel<float, 1, true>,
-                                      (const void*)iso3dfd_direct_kernel<float, 2, true>},
-                                     {(const void*)iso3dfd_direct_kernel<double, 0, true>, (const void*)iso3dfd_direct_kernel<double, 1, true>,
-                                      (const void*)iso3dfd_direct_kernel<double, 2, true>}};
-            for (int m = 0; m < 3; m++) preload_kernel(fns[f64][m]);
-        } else if (f64) {
-            preload_kernel((const void*)iso3dfd_direct_kernel<double, 0>);
-            preload_kernel((const void*)iso3dfd_direct_kernel<double, 1>);
-            preload_kernel((const void*)iso3dfd_direct_kernel<double, 2>);
-        } else {
-            preload_kernel((const void*)iso3dfd_direct_kernel<float, 0>);
-            preload_kernel((const void*)iso3dfd_direct_kernel<float, 1>);
-            preload_kernel((const void*)iso3dfd_direct_kernel<float, 2>);
-        }
+        for (int m = 0; m < 3; m++)
+            preload_kernel(f64 ? (const void*)direct_kernel<double>(sponge, m) : (const void*)direct_kernel<float>(sponge, m));
         return 0;
     }
 
-    // Tensor maps of one sweep variant with p(t) in slot `cur`.
     template <class E>
-    static int make_maps(const Solution& s, const TileCfgT<E>& c, int cur, IsoMaps& m) {
-        const Var& p = s.vars[0];
-        const Var& v = s.vars[1];
-        if (int rc = make_map(&m.h, p, cur, c.hp, c.hrows)) return rc;
-        if (int rc = make_map(&m.c, p, cur, c.tz, c.ty)) return rc;
-        if (int rc = make_map(&m.p, p, cur ^ 1, c.tz, c.ty)) return rc;
-        return make_map(&m.v, v, 0, c.tz, c.ty);
+    std::vector<IsoSweep<E>>& sweeps() {
+        if constexpr (sizeof(E) == 8) return sweeps_f64;
+        else return sweeps_f32;
     }
 
-    // The sweep variant a launch uses: the selected tile (in its resident-plane form where it has one and `resident` is on) at
-    // radius 8, the one compiled variant at other radii, in fp64 and for iso3dfd_sponge (which has no fp32 radius-8 form).
-    bool resident_on() const { return radius == 8 && !f64 && !sponge && resident && resident_cfg(tile); }
+    // The one-step sweep forms this solution can launch, with their tensor maps for every slot of p(t): at radius 8 in fp32 the
+    // resident-plane forms, then every tile; the one compiled form of the radius elsewhere (fp64 and iso3dfd_sponge have no
+    // radius-8 fp32 form).  The selected form is loaded now.
     template <class E>
-    const TileCfgT<E>& sweep_cfg() const {
-        if constexpr (sizeof(E) == 8) return sponge ? *iso_sponge_cfg_f64(radius) : *iso_radius_cfg_f64(radius);
-        else if (sponge) return *iso_sponge_cfg(radius);
-        else return radius != 8 ? *iso_radius_cfg(radius) : resident_on() ? *resident_cfg(tile) : tile_cfg(tile);
+    int build_sweeps(const Solution& s, int nsl) {
+        std::vector<IsoSweep<E>>& ws = sweeps<E>();
+        if constexpr (sizeof(E) == 8) ws.push_back({{sponge ? iso_sponge_cfg_f64(radius) : iso_radius_cfg_f64(radius)}, -1, false});
+        else if (radius != 8 || sponge) ws.push_back({{sponge ? iso_sponge_cfg(radius) : iso_radius_cfg(radius)}, -1, false});
+        else {
+            for (int tl = 0; tl < NTILES; tl++)
+                if (const TileCfg* c = resident_cfg(tl)) ws.push_back({{c}, tl, true});
+            for (int tl = 0; tl < NTILES; tl++) ws.push_back({{&tile_cfg(tl)}, tl, false});
+        }
+        const Var& p = s.vars[0];
+        const Var& v = s.vars[1];
+        for (IsoSweep<E>& w : ws)
+            for (int cur = 0; cur < nsl; cur++) {
+                const TileCfgT<E>& c = *w.cfg;
+                IsoMaps& m = w.maps[cur];
+                if (int rc = make_var_tensor_map(&m.h, p, cur, c.hp, c.hrows)) return rc;
+                if (int rc = make_var_tensor_map(&m.c, p, cur, c.tz, c.ty)) return rc;
+                if (int rc = make_var_tensor_map(&m.p, p, cur ^ 1, c.tz, c.ty)) return rc;
+                if (int rc = make_var_tensor_map(&m.v, v, 0, c.tz, c.ty)) return rc;
+            }
+        for (int m = 0; m < 4; m++) preload_kernel((const void*)sweep<E>().cfg->fn[m]);
+        return 0;
     }
-    // Row of attr_set: the tile at radius 8 (NTILES + 0 / 1: resident forms of tiles 6 / 7), 0 otherwise.
-    int cfg_index() const { return radius != 8 ? 0 : resident_on() ? NTILES + (tile == 7) : tile; }
+
+    // The sweep form a launch uses: the first whose tile is the selected one (or any) and which `resident` allows, i.e. the
+    // resident-plane form of the tile where it has one and `resident` is on.
+    template <class E>
+    IsoSweep<E>& sweep() {
+        std::vector<IsoSweep<E>>& ws = sweeps<E>();
+        for (IsoSweep<E>& w : ws)
+            if ((w.tile < 0 || w.tile == tile) && (resident || !w.resident)) return w;
+        return ws.front();      // not reached: every tile has a plain form
+    }
 
     template <class E>
     void fill_params(const Solution& s, int64_t t, const Box& box, IsoParamsT<E>& P) const {
@@ -549,13 +559,13 @@ struct IsoEngine : Engine {
             use_tma = false;
         }
         if (use_tma) {
-            const int ti = (radius == 8 && !f64 && !sponge) ? tile : 0;      // tensor maps; other radii, fp64 and sponge: one compiled variant
-            const int ai = cfg_index();
-            const TileCfgT<E>& c = sweep_cfg<E>();
+            IsoSweep<E>& w = sweep<E>();
+            const TileCfgT<E>& c = *w.cfg;
             if (mem_probe && c.fn[3]) mode = 3;
-            // fused halo exchange: only for whole-domain launches of a kernel that implements the peer stores
+            // fused halo exchange: only for whole-domain launches of a kernel that implements the peer stores (fp32: FUSED in
+            // the kernels)
             P.peer_lo = P.peer_hi = nullptr;
-            bool fused = s.fused_x.var == 0 && c.fused_ok && mode != 3 && box.b[0] == 0 && box.e[0] == P.nx && P.nx >= 2 * radius;
+            bool fused = s.fused_x.var == 0 && sizeof(E) == 4 && mode != 3 && box.b[0] == 0 && box.e[0] == P.nx && P.nx >= 2 * radius;
             // in-kernel completion signal: needs room for boundary-first chunks; the copy-engine path exists only with it
             const bool sig = fused && s.fused_x.counter != nullptr && P.nx >= 4 * radius;
             if (fused && s.fused_x.dma && !sig) fused = false;
@@ -571,47 +581,15 @@ struct IsoEngine : Engine {
             P.ntz = int((box.e[2] - box.b[2] + c.tz - 1) / c.tz);
             const int64_t ntile = int64_t(P.nty) * P.ntz;
             const int gmax = grid_override > 0 ? grid_override : num_sms;
-            // x chunks of equal length.  With an in-kernel completion signal the chunk that starts at plane 0 and the chunk
-            // that ends at plane nx-1 (swept downwards) are numbered first, so that every CTA computes -- and stores into the
-            // neighbours -- the boundary planes at the very start of its first sweeps.
-            const int64_t ib = box.b[0], ie = box.e[0];
-            const int64_t nxb = ie - ib;
-            const int min_nc = (sig && nb_lo && nb_hi) ? 2 : 1;
-            const int64_t max_nc = std::min<int64_t>(ISO_MAX_CHUNKS, sig ? nxb / radius : nxb);
-            int nc_best = min_nc;
-            if (lx > 0) {
-                nc_best = int(std::max<int64_t>(min_nc, std::min<int64_t>((nxb + lx - 1) / lx, max_nc)));
-            } else {
-                // Pick the chunk count that minimises (rounds of units per CTA) x (chunk length + queue
-                // warm-up): long chunks amortise the 2R warm-up planes, short ones balance the last round.
-                double best = 1e30;
-                for (int64_t nc = min_nc; nc <= max_nc; nc++) {
-                    const int64_t l = (nxb + nc - 1) / nc;
-                    const int64_t rounds = (ntile * nc + gmax - 1) / gmax;
-                    const double cost = double(rounds) * (double(l) + 2 * radius * 0.4);
-                    if (cost < best * 0.999) { best = cost; nc_best = int(nc); }
-                }
-            }
-            int nb = 0, nsig = 0;
-            {
-                const int nc = nc_best;      // balanced partition: chunk lengths differ by at most one plane (all >= R when signalling)
-                std::vector<int> order;
-                if (sig && nb_lo) order.push_back(0);
-                if (sig && nb_hi && !(nc == 1 && nb_lo)) order.push_back(nc - 1);
-                nsig = int(order.size());
-                for (int c = 0; c < nc; c++)
-                    if (std::find(order.begin(), order.end(), c) == order.end()) order.push_back(c);
-                for (int c : order) {
-                    const int64_t x0 = ib + nxb * c / nc, x1 = ib + nxb * (c + 1) / nc;
-                    const bool down = sig && nb_hi && c == nc - 1 && !(nc == 1 && nb_lo);
-                    P.cx0[nb] = int(down ? x1 - 1 : x0); P.clen[nb] = int(x1 - x0); P.cdir[nb] = down ? -1 : 1;
-                    nb++;
-                }
-            }
-            P.nchunks = nb;
+            // x chunks of equal length, each at least R planes long when signalling.  With an in-kernel completion signal the chunk
+            // that starts at plane 0 and the chunk that ends at plane nx-1 (swept downwards) are numbered first, so that every CTA
+            // computes -- and stores into the neighbours -- the boundary planes at the very start of its first sweeps.
+            const int64_t nxb = box.e[0] - box.b[0];
+            P.nchunks = chunk_count(nxb, ntile, gmax, lx, 2 * radius, (sig && nb_lo && nb_hi) ? 2 : 1,
+                                    std::min<int64_t>(ISO_MAX_CHUNKS, sig ? nxb / radius : nxb));
+            const int nsig = chunk_partition(box.b[0], nxb, P.nchunks, sig && nb_lo, sig && nb_hi, P.cx0, P.clen, P.cdir);
             P.sig_units = 0; P.sig_total = 0; P.sig_counter = nullptr; P.sig_flag_lo = P.sig_flag_hi = nullptr; P.sig_epoch = 0;
-            const int64_t nunits = int64_t(P.nty) * P.ntz * P.nchunks;
-            int grid = int(std::min<int64_t>(nunits, gmax));
+            const int grid = int(std::min<int64_t>(ntile * P.nchunks, gmax));
             if (sig) {
                 P.sig_units = int(ntile) * nsig;
                 P.sig_total = unsigned(grid) * unsigned(c.ty * c.tz / (2 * IsoVec<E>::N) / 32);   // consumer warps: 2 vectors per thread
@@ -620,28 +598,13 @@ struct IsoEngine : Engine {
                 P.sig_epoch = s.fused_x.epoch;
                 s.fused_x.signalled = true;
             }
-            if (!attr_set[ai][mode]) {
-                YB_CUDA(cudaFuncSetAttribute(c.fn[mode], cudaFuncAttributeMaxDynamicSharedMemorySize, int(c.smem)));
-                attr_set[ai][mode] = true;
-            }
-            c.fn[mode]<<<grid, c.threads, c.smem, st>>>(maps[ti][cur], P);
+            if (int rc = w.launch(mode, cur, grid, P, st)) return rc;
         } else {
             dim3 blk(128, 1, 1);
             dim3 grd(unsigned((box.e[2] - box.b[2] + 127) / 128), unsigned(box.e[1] - box.b[1]), unsigned(box.e[0] - box.b[0]));
             if (grd.y > 65535 || grd.z > 65535) return set_error(YB_EUNSUPPORTED, "direct kernel: domain too large in x or y");
-            if (sponge) {
-                switch (mode) {
-                    case 0: iso3dfd_direct_kernel<E, 0, true><<<grd, blk, 0, st>>>(P, radius); break;
-                    case 1: iso3dfd_direct_kernel<E, 1, true><<<grd, blk, 0, st>>>(P, radius); break;
-                    default: iso3dfd_direct_kernel<E, 2, true><<<grd, blk, 0, st>>>(P, radius); break;
-                }
-            } else {
-                switch (mode) {
-                    case 0: iso3dfd_direct_kernel<E, 0><<<grd, blk, 0, st>>>(P, radius); break;
-                    case 1: iso3dfd_direct_kernel<E, 1><<<grd, blk, 0, st>>>(P, radius); break;
-                    default: iso3dfd_direct_kernel<E, 2><<<grd, blk, 0, st>>>(P, radius); break;
-                }
-            }
+            const DirectFn<E> fn = direct_kernel<E>(sponge, mode == 0 || mode == 1 ? mode : 2);
+            fn<<<grd, blk, 0, st>>>(P, radius);
         }
         YB_CUDA(cudaGetLastError());
         return 1;
@@ -688,8 +651,8 @@ struct IsoEngine : Engine {
     int launch_steps(Solution& s, int64_t t, int nsteps, const Box& box, cudaStream_t st) override {
         if (nsteps != 2 || !tt_ok) return set_error(YB_EUNSUPPORTED, "iso3dfd: no temporal tile for %d steps in this configuration", nsteps);
         if (box.empty()) return 0;
-        const int vr = tt_var();
-        const TTCfg& c = *tt_radius_cfg(radius, vr);
+        SweepForm<TTCfg, TTMaps>& w = tts[tt_var()];
+        const TTCfg& c = *w.cfg;
         Var& p = s.vars[0];
         const Var& v = s.vars[1];
         const Dim *px = p.domain_dim(0), *py = p.domain_dim(1), *pz = p.domain_dim(2);
@@ -713,35 +676,13 @@ struct IsoEngine : Engine {
         P.pol_p = pol_h; P.st_cs = st_cs;       // same options (pol_h, st_cs) and defaults as the one-step kernel's haloed p(t) stream / stores
         P.nty = (P.ny + c.ty - 1) / c.ty;
         P.ntz = (P.nz + c.tz - 1) / c.tz;
-        // x chunks of (almost) equal length: minimise (rounds of units per CTA) x (chunk length + warm-up iterations;
-        // those of the first 2R only load, the next 2R only run step 1)
+        // x chunks of (almost) equal length; of a chunk's warm-up iterations the first 2R only load, the next 2R only run step 1
         const int64_t ntile = int64_t(P.nty) * P.ntz;
         const int gmax = grid_override > 0 ? grid_override : num_sms;
-        const int64_t max_nc = std::min<int64_t>(TT_MAX_CHUNKS, P.nx);
-        int nc_best = 1;
-        if (lx > 0) nc_best = int(std::max<int64_t>(1, std::min<int64_t>((P.nx + lx - 1) / lx, max_nc)));
-        else {
-            double best = 1e30;
-            for (int64_t nc = 1; nc <= max_nc; nc++) {
-                const int64_t l = (P.nx + nc - 1) / nc;
-                const int64_t rounds = (ntile * nc + gmax - 1) / gmax;
-                const double cost = double(rounds) * (double(l) + c.warm * 0.4);
-                if (cost < best * 0.999) { best = cost; nc_best = int(nc); }
-            }
-        }
-        P.nchunks = nc_best;
-        for (int k = 0; k < nc_best; k++) {
-            const int64_t x0 = int64_t(P.nx) * k / nc_best, x1 = int64_t(P.nx) * (k + 1) / nc_best;
-            P.cx0[k] = int(x0); P.clen[k] = int(x1 - x0);
-        }
-        const int64_t nunits = ntile * P.nchunks;
-        const int grid = int(std::min<int64_t>(nunits, gmax));
-        const int mode = std::min(std::max(s.fp_mode, 0), 2);
-        if (!tt_attr_set[vr][mode]) {
-            YB_CUDA(cudaFuncSetAttribute(c.fn[mode], cudaFuncAttributeMaxDynamicSharedMemorySize, int(c.smem)));
-            tt_attr_set[vr][mode] = true;
-        }
-        c.fn[mode]<<<grid, c.threads, c.smem, st>>>(tt_maps[cur], P);
+        P.nchunks = chunk_count(P.nx, ntile, gmax, lx, c.warm, 1, std::min<int64_t>(TT_MAX_CHUNKS, P.nx));
+        chunk_partition(0, P.nx, P.nchunks, false, false, P.cx0, P.clen, nullptr);
+        const int grid = int(std::min<int64_t>(ntile * P.nchunks, gmax));
+        if (int rc = w.launch(std::min(std::max(s.fp_mode, 0), 2), cur, grid, P, st)) return rc;
         YB_CUDA(cudaGetLastError());
         tt_launches++;
         p.slot_bias ^= 2;       // steps t+1, t+2 (and every later access, stream-ordered) live in the other pair now
@@ -756,12 +697,35 @@ struct IsoEngine : Engine {
         tile = TUNE_TILES[v / 3]; lx = TUNE_LXS[v % 3];
         s.options["tile"] = std::to_string(tile);
         s.options["lx"] = std::to_string(lx);
-        preload_kernel((const void*)sweep_cfg<float>().fn[s.fp_mode]);
+        preload_kernel((const void*)sweep<float>().cfg->fn[s.fp_mode]);
     }
     std::string tune_describe(const Solution&, int v) const override {
         char b[160];
         snprintf(b, sizeof b, "tile=%d (%s) lx=%d", TUNE_TILES[v / 3], tile_cfg(TUNE_TILES[v / 3]).name, TUNE_LXS[v % 3]);
         return b;
+    }
+
+    // Trial loop of the offline tuners: trial(i, line) applies candidate i, times it (ms per step, < 0 when a launch failed) and
+    // writes its report line.  Sets best to the fastest candidate and best_ms to its time; after a failed launch every option
+    // the tuners change is restored and the error returned.
+    template <class F>
+    int tune_trials(int n, std::string& report, int& best, double& best_ms, F trial) {
+        const int keep_tile = tile, keep_lx = lx, keep_bs = block_steps, keep_var = tt_variant;
+        const bool keep_res = resident;
+        char line[200];
+        report.clear();
+        best = 0;
+        best_ms = 1e30;
+        for (int i = 0; i < n; i++) {
+            const double ms = trial(i, line);
+            if (ms < 0) {
+                tile = keep_tile; resident = keep_res; lx = keep_lx; block_steps = keep_bs; tt_variant = keep_var;
+                return set_error(YB_ECUDA, "auto-tuner: a trial launch failed");
+            }
+            report += line;
+            if (ms < best_ms) { best_ms = ms; best = i; }
+        }
+        return 0;
     }
 
     // Offline tuner of a solution that has a temporal tile: one step per sweep against two steps per sweep in each compiled form,
@@ -771,28 +735,25 @@ struct IsoEngine : Engine {
         for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = s.rank_size[d]; }
         int64_t t = s.vars[0].last_valid_step();
         if (int rc = begin_run(s, t, st)) return rc;
-        const int keep_bs = block_steps, keep_var = tt_variant;
         const int dflt_var = tt_var();
-        double best = 1e30;
-        int best_bs = 1, best_var = tt_var();
-        char line[200];
-        report.clear();
-        for (int cand = 0; cand <= TT_VARIANTS; cand++) {
-            double ms;
-            if (cand == 0) {
-                ms = time_launches(st, 4, [&]() { return launch(s, 0, t++, whole, st); });
-                snprintf(line, sizeof line, " one step per sweep: %.4f ms/step\n", ms);
-            } else {
+        int best;
+        double best_ms;
+        if (int rc = tune_trials(TT_VARIANTS + 1, report, best, best_ms, [&](int cand, auto& line) {
+                if (cand == 0) {
+                    const double ms = time_launches(st, 4, [&]() { return launch(s, 0, t++, whole, st); });
+                    snprintf(line, sizeof line, " one step per sweep: %.4f ms/step\n", ms);
+                    return ms;
+                }
                 tt_variant = cand - 1;
-                ms = time_launches(st, 3, [&]() { const int rc = launch_steps(s, t, 2, whole, st); t += 2; return rc; }) / 2;
-                snprintf(line, sizeof line, " two steps per sweep, %s: %.4f ms/step\n", tt_radius_cfg(radius, tt_variant)->name, ms);
-            }
-            if (ms < 0) { block_steps = keep_bs; tt_variant = keep_var; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-            report += line;
-            if (ms < best) { best = ms; best_bs = cand == 0 ? 1 : 2; best_var = cand == 0 ? dflt_var : cand - 1; }
-        }
-        block_steps = best_bs; tt_variant = best_var;
-        snprintf(line, sizeof line, "best: block_steps=%d tt_variant=%d (%.4f ms/step)\n", block_steps, tt_variant, best);
+                const double ms = time_launches(st, 3, [&]() { const int rc = launch_steps(s, t, 2, whole, st); t += 2; return rc; }) / 2;
+                snprintf(line, sizeof line, " two steps per sweep, %s: %.4f ms/step\n", tts[tt_variant].cfg->name, ms);
+                return ms;
+            }))
+            return rc;
+        block_steps = best == 0 ? 1 : 2;
+        tt_variant = best == 0 ? dflt_var : best - 1;
+        char line[200];
+        snprintf(line, sizeof line, "best: block_steps=%d tt_variant=%d (%.4f ms/step)\n", block_steps, tt_variant, best_ms);
         report += line;
         s.options["block_steps"] = std::to_string(block_steps);
         s.options["tt_variant"] = std::to_string(tt_variant);
@@ -807,35 +768,37 @@ struct IsoEngine : Engine {
     int auto_tune(Solution& s, cudaStream_t st, std::string& report) override {
         if (tt_ok && kernel != "direct" && !s.multi_rank()) return auto_tune_temporal(s, st, report);
         if (!maps_ok || (radius != 8 && !f64) || kernel == "direct") { report = "iso3dfd: no tiled variants to tune for this configuration"; return 0; }
+        return f64 ? auto_tune_sweep<double>(s, st, report) : auto_tune_sweep<float>(s, st, report);
+    }
+    template <class E>
+    int auto_tune_sweep(Solution& s, cudaStream_t st, std::string& report) {
         Box whole;
         for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = s.rank_size[d]; }
         if (whole.e[1] < 8 || whole.e[2] < 16) { report = "iso3dfd: domain too thin for the tiled kernel"; return 0; }
         const int64_t t0 = s.vars[0].last_valid_step();
         // (tile, resident) pairs; resident = 1 only where the tile has a resident-plane form
         const std::vector<std::pair<int, bool>> forms =
-            f64 ? std::vector<std::pair<int, bool>>{{tile, false}}
-                : std::vector<std::pair<int, bool>>{{7, true}, {6, true}, {7, false}, {6, false}, {5, false}, {4, false}, {1, false}, {0, false}};
-        const int lxs[] = {0, 256, 512, 1024};   // planes per interior chunk (0 = cost model)
-        const int keep_tile = tile, keep_lx = lx;
-        const bool keep_res = resident;
-        double best = 1e30;
-        int best_tile = tile, best_lx = lx;
-        bool best_res = resident;
-        char line[160];
-        report.clear();
+            sizeof(E) == 8 ? std::vector<std::pair<int, bool>>{{tile, false}}
+                           : std::vector<std::pair<int, bool>>{{7, true}, {6, true}, {7, false}, {6, false}, {5, false}, {4, false}, {1, false}, {0, false}};
+        struct Cand { int tile; bool resident; int lx; };
+        std::vector<Cand> cands;
         for (const auto& [ti, res] : forms)
-            for (int l : lxs) {
-                if (l > whole.e[0]) continue;
-                tile = ti; resident = res; lx = l;
+            for (int l : {0, 256, 512, 1024})       // planes per interior chunk (0 = cost model)
+                if (l <= whole.e[0]) cands.push_back({ti, res, l});
+        int best;
+        double best_ms;
+        if (int rc = tune_trials(int(cands.size()), report, best, best_ms, [&](int i, auto& line) {
+                tile = cands[i].tile; resident = cands[i].resident; lx = cands[i].lx;
                 int64_t t = t0;
                 const double ms = time_launches(st, 3, [&]() { return launch(s, 0, t++, whole, st); });
-                if (ms < 0) { tile = keep_tile; resident = keep_res; lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-                snprintf(line, sizeof line, " tile=%d resident=%d (%s) lx=%d: %.4f ms/step\n", ti, int(resident_on()), f64 ? sweep_cfg<double>().name : sweep_cfg<float>().name, l, ms);
-                report += line;
-                if (ms < best) { best = ms; best_tile = ti; best_res = res; best_lx = l; }
-            }
-        tile = best_tile; resident = best_res; lx = best_lx;
-        snprintf(line, sizeof line, "best: tile=%d resident=%d lx=%d (%.4f ms/step)\n", tile, int(resident_on()), lx, best);
+                const IsoSweep<E>& w = sweep<E>();
+                snprintf(line, sizeof line, " tile=%d resident=%d (%s) lx=%d: %.4f ms/step\n", tile, int(w.resident), w.cfg->name, lx, ms);
+                return ms;
+            }))
+            return rc;
+        tile = cands[best].tile; resident = cands[best].resident; lx = cands[best].lx;
+        char line[200];
+        snprintf(line, sizeof line, "best: tile=%d resident=%d lx=%d (%.4f ms/step)\n", tile, int(sweep<E>().resident), lx, best_ms);
         report += line;
         s.options["tile"] = std::to_string(tile);
         s.options["resident"] = resident ? "1" : "0";

@@ -243,8 +243,8 @@ __device__ __forceinline__ void arr_to_v(const double* a, double2& v) { v = make
 //   pv, v   row a in the p(t-1) and v tiles (T::TZ elements per row)
 //   oa      row a's output vector; row b is P.out_sy further on
 // Results leave as 128-bit stores where the row's vector is whole and aligned (scalars on ragged edges).  The fused halo
-// exchange (peer stores into the x neighbours' halo cells) is compiled for fp32 only: the fp64 sweep is listed with
-// fused_ok = false, and leaving the out-of-line signal call out keeps its registers free of call spills.
+// exchange (peer stores into the x neighbours' halo cells) is compiled for fp32 only: the engine never fuses an fp64
+// sweep, and leaving the out-of-line signal call out keeps its registers free of call spills.
 // SP (iso3dfd_sponge): both rows' results are scaled by the sponge factors in `sg` (iso_sponge) before every store, the peer
 // stores included.
 template <class E>

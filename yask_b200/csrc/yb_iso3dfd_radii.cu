@@ -5,20 +5,12 @@
 
 namespace yb {
 
-namespace {
-template <int R>
-TileCfg make_cfg(const char* name) {
-    using T = IsoTile2<R, 8, 32, 5>;
-    return TileCfg{true, name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128, T::SMEM_BYTES,
-                   {iso3dfd_tma2_kernel<T, 0, 1, 2>, iso3dfd_tma2_kernel<T, 1, 1, 2>, iso3dfd_tma2_kernel<T, 2, 1, 2>, nullptr}};
-}
-}  // namespace
-
 const TileCfg* iso_radius_cfg(int radius) {
-    static const TileCfg cfgs[7] = {make_cfg<1>("r1 16x128 PW U2"), make_cfg<2>("r2 16x128 PW U2"), make_cfg<3>("r3 16x128 PW U2"),
-                                    make_cfg<4>("r4 16x128 PW U2"), make_cfg<5>("r5 16x128 PW U2"), make_cfg<6>("r6 16x128 PW U2"),
-                                    make_cfg<7>("r7 16x128 PW U2")};
-    return (radius >= 1 && radius <= 7) ? &cfgs[radius - 1] : nullptr;
+    static const TileCfg cfgs[7] = {iso_default_cfg<1, float>("r1 16x128 PW U2"), iso_default_cfg<2, float>("r2 16x128 PW U2"),
+                                    iso_default_cfg<3, float>("r3 16x128 PW U2"), iso_default_cfg<4, float>("r4 16x128 PW U2"),
+                                    iso_default_cfg<5, float>("r5 16x128 PW U2"), iso_default_cfg<6, float>("r6 16x128 PW U2"),
+                                    iso_default_cfg<7, float>("r7 16x128 PW U2")};
+    return iso_cfg_of_radius(cfgs, radius);
 }
 
 }  // namespace yb

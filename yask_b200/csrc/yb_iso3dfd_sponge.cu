@@ -6,22 +6,13 @@
 
 namespace yb {
 
-namespace {
-template <int R>
-TileCfg make_sponge_cfg(const char* name) {
-    using T = IsoTile2<R, 8, 32, 5>;
-    return TileCfg{true, name, T::TY, T::TZ, T::HP, T::HROWS, T::THREADS + 128, T::SMEM_BYTES,
-                   {iso3dfd_tma2_kernel<T, 0, 1, 2, true>, iso3dfd_tma2_kernel<T, 1, 1, 2, true>, iso3dfd_tma2_kernel<T, 2, 1, 2, true>,
-                    nullptr}};
-}
-}  // namespace
-
 const TileCfg* iso_sponge_cfg(int radius) {
-    static const TileCfg cfgs[7] = {make_sponge_cfg<1>("sponge r1 16x128 PW U2"), make_sponge_cfg<2>("sponge r2 16x128 PW U2"),
-                                    make_sponge_cfg<3>("sponge r3 16x128 PW U2"), make_sponge_cfg<4>("sponge r4 16x128 PW U2"),
-                                    make_sponge_cfg<5>("sponge r5 16x128 PW U2"), make_sponge_cfg<6>("sponge r6 16x128 PW U2"),
-                                    make_sponge_cfg<7>("sponge r7 16x128 PW U2")};
-    return (radius >= 1 && radius <= 7) ? &cfgs[radius - 1] : nullptr;
+    static const TileCfg cfgs[7] = {
+        iso_default_cfg<1, float, true>("sponge r1 16x128 PW U2"), iso_default_cfg<2, float, true>("sponge r2 16x128 PW U2"),
+        iso_default_cfg<3, float, true>("sponge r3 16x128 PW U2"), iso_default_cfg<4, float, true>("sponge r4 16x128 PW U2"),
+        iso_default_cfg<5, float, true>("sponge r5 16x128 PW U2"), iso_default_cfg<6, float, true>("sponge r6 16x128 PW U2"),
+        iso_default_cfg<7, float, true>("sponge r7 16x128 PW U2")};
+    return iso_cfg_of_radius(cfgs, radius);
 }
 
 }  // namespace yb
