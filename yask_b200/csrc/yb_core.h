@@ -283,6 +283,11 @@ int make_var_tensor_map(void* map, const Var& v, int slot, int box_z, int box_y)
 // engines
 std::unique_ptr<Engine> make_iso3dfd_engine();
 StencilSpec iso3dfd_spec(int radius, int elem_bytes, bool sponge);
+// 3axis, 3axis_with_diags, 3plane, cube (yb_avepts.cu): shape index 0..3 of a solution name (-1: none of them), points read
+std::unique_ptr<Engine> make_avepts_engine();
+int avepts_shape(const std::string& name);
+int64_t avepts_points(int shape, int radius);
+StencilSpec avepts_spec(int shape, int radius, int elem_bytes);
 
 // device utilities (yb_fill.cu)
 struct BoxCopy {

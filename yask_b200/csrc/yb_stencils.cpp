@@ -58,6 +58,19 @@ int registry_create(const std::string& name, int radius, int elem_bytes, Stencil
         eng = make_iso3dfd_engine();
         return 0;
     }
+    if (const int shape = avepts_shape(name); shape >= 0) {
+        // 3axis, 3axis_with_diags, 3plane and cube: the emitter generated them in fp32 at the reference's default radii (4, 4, 3
+        // and 2: the constructors' defaults in its src/stencils/SimpleStencils.cpp), which stay on those kernels.  Every other radius up
+        // to 8, and every radius in fp64, takes the hand-written average-of-points sweep (yb_avepts.cu).
+        static const int default_radius[4] = {4, 4, 3, 2};
+        if (radius > 8) return set_error(YB_EUNSUPPORTED, "%s: radius %d > 8 is not supported", name.c_str(), radius);
+        const int eb = elem_bytes == 0 ? 4 : elem_bytes;
+        if (eb != 4 && eb != 8) return set_error(YB_EUNSUPPORTED, "%s: elements must be 4 or 8 bytes", name.c_str());
+        if (eb == 4 && (radius <= 0 || radius == default_radius[shape])) return gen_registry_create(name, elem_bytes, spec, eng);
+        spec = avepts_spec(shape, radius <= 0 ? default_radius[shape] : radius, eb);
+        eng = make_avepts_engine();
+        return 0;
+    }
     int rc = gen_registry_create(name, elem_bytes, spec, eng);
     if (rc != YB_EINVAL) return rc;
     return set_error(YB_EINVAL, "unknown stencil solution '%s'", name.c_str());

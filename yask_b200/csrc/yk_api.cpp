@@ -469,20 +469,29 @@ struct B200Solution : yk_solution {
     // The reference fixes a solution's radius and element size when it builds the kernel library (`make stencil=iso3dfd
     // radius=2 real_bytes=8`, /root/reference/src/kernel/Makefile); here the library name carries them the same way:
     // libyask_kernel.iso3dfd_r2.b200.so (-DYK_STENCIL_NAME=iso3dfd_r2) is iso3dfd with radius 2, and a `_fp64` suffix
-    // (iso3dfd_r4_fp64) selects 8-byte elements; iso3dfd_sponge_r<N>[_fp64] does the same for iso3dfd_sponge.
-    // YASK_B200_RADIUS and YASK_B200_ELEM_BYTES override them at run time.
+    // (iso3dfd_r4_fp64) selects 8-byte elements; iso3dfd_sponge_r<N>[_fp64], 3axis_r<N>[_fp64], 3axis_with_diags_r<N>[_fp64],
+    // 3plane_r<N>[_fp64] and cube_r<N>[_fp64] do the same for those solutions.  YASK_B200_RADIUS and YASK_B200_ELEM_BYTES override
+    // them at run time.
+    static bool takes_radius(const std::string& base) {
+        for (const char* n : {"iso3dfd", "iso3dfd_sponge", "3axis", "3axis_with_diags", "3plane", "cube"})
+            if (base == n) return true;
+        return false;
+    }
     explicit B200Solution(const char* stencil_) {
         std::string stencil = stencil_;
         int radius = 0, elem_bytes = 0;
-        const std::string fp64 = "_fp64";      // iso3dfd_fp64, iso3dfd_r<N>_fp64, iso3dfd_sponge_r<N>_fp64
-        if (stencil.size() > fp64.size() && stencil.compare(stencil.size() - fp64.size(), fp64.size(), fp64) == 0 &&
-            (stencil.compare(0, 9, "iso3dfd_r") == 0 || stencil.compare(0, 16, "iso3dfd_sponge_r") == 0 || stencil == "iso3dfd" + fp64)) {
-            elem_bytes = 8;
-            stencil.resize(stencil.size() - fp64.size());
+        const std::string fp64 = "_fp64";      // iso3dfd_fp64, <solution>_r<N>_fp64
+        if (stencil.size() > fp64.size() && stencil.compare(stencil.size() - fp64.size(), fp64.size(), fp64) == 0) {
+            const std::string base = stencil.substr(0, stencil.size() - fp64.size());
+            const size_t r = base.rfind("_r");
+            if (base == "iso3dfd" || (r != std::string::npos && r + 2 < base.size() && takes_radius(base.substr(0, r)) &&
+                                      base.find_first_not_of("0123456789", r + 2) == std::string::npos)) {
+                elem_bytes = 8;
+                stencil = base;
+            }
         }
         const size_t us = stencil.rfind("_r");
-        if (us != std::string::npos && us + 2 < stencil.size() &&
-            (stencil.compare(0, us, "iso3dfd") == 0 || stencil.compare(0, us, "iso3dfd_sponge") == 0) &&
+        if (us != std::string::npos && us + 2 < stencil.size() && takes_radius(stencil.substr(0, us)) &&
             stencil.find_first_not_of("0123456789", us + 2) == std::string::npos) {
             radius = atoi(stencil.c_str() + us + 2);
             stencil.resize(us);
