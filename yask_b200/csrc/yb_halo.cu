@@ -30,7 +30,7 @@ namespace yb {
 namespace {
 
 constexpr uint32_t BLOB_MAGIC = 0x59423230;  // "YB20"
-constexpr int MAX_VARS = 32;
+constexpr int MAX_VARS = 128;    // vars of one solution a blob describes (fsg_abc declares 70)
 constexpr int NDIRS = 27;
 
 struct BlobVar {
@@ -651,7 +651,7 @@ int yb_halo_export(yb_solution* s_, void* out, size_t nbytes) {
     YB_CUDA(cudaSetDevice(s->device));
     Blob b;
     memset(&b, 0, sizeof b);
-    b.magic = BLOB_MAGIC; b.version = 3; b.pid = int64_t(getpid()); b.nonce = process_nonce(); b.device = s->device;
+    b.magic = BLOB_MAGIC; b.version = 4; b.pid = int64_t(getpid()); b.nonce = process_nonce(); b.device = s->device;
     b.num_vars = int(s->vars.size());
     for (int k = 0; k < 3; k++) { b.rank_index[k] = s->rank_index[k]; b.rank_size[k] = s->rank_size[k]; }
     b.fused_steps = s->engine->fused_steps(*s);
