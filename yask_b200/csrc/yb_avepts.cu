@@ -77,6 +77,25 @@ const AvpCfgT<E>* sweep_cfg(int shape, int R) {
     return nullptr;
 }
 
+// The temporal tile of (shape, radius, element size), or null where block_steps has no effect.
+template <class E>
+const AvpTTCfgT<E>* tt_cfg(int shape, int R) {
+    if (R < 1 || R > AVP_TT_MAX_R) return nullptr;
+    const AvpTTCfgT<E>* t = nullptr;
+    switch (shape) {
+        case AVP_3AXIS: t = avp_tt_table<AVP_3AXIS, E>(); break;
+        case AVP_DIAGS: t = avp_tt_table<AVP_DIAGS, E>(); break;
+        case AVP_PLANE: t = avp_tt_table<AVP_PLANE, E>(); break;
+        case AVP_CUBE: t = avp_tt_table<AVP_CUBE, E>(); break;
+        default: return nullptr;
+    }
+    return t[R - 1].fn ? &t[R - 1] : nullptr;
+}
+bool has_tt(const StencilSpec& sp) {
+    const int shape = avepts_shape(sp.name);
+    return sp.elem_bytes == 8 ? tt_cfg<double>(shape, sp.radius) != nullptr : tt_cfg<float>(shape, sp.radius) != nullptr;
+}
+
 template <class E>
 using AvpDirectFn = void (*)(AvpParamsT<E>, int);
 template <class E>
@@ -101,11 +120,21 @@ struct AvpEngine : Engine {
     int lx = 0;                    // planes per sweep chunk (0 = cost model)
     int grid_override = 0;
     int gmax = 132;                // resident CTAs of the sweep kernel over the device
+    int tt_gmax = 132;             // the same for the temporal tile
+    int num_sms = 132;
     bool maps_ok = false, attr_set = false;
-    CUtensorMap maps[2];           // A(t) in each step slot
+    CUtensorMap maps[4];           // A(t) in each storage slot (4 with the temporal tile's spare pair)
+    // Temporal tile: option block_steps (the reference's -bt).  Its spare pair of slots is planned at prepare (plan_storage), so the
+    // option must be set before prepare_solution(); later changes only switch the launch path.  One rank only.
+    int block_steps = 1;
+    int64_t tt_launches = 0;       // read-only option tt_launches: fused launches since prepare
+    bool tt_ok = false;            // spare slots allocated and tensor maps built
+    CUtensorMap tt_maps[4];        // A(t) in each storage slot, the tile's boxes
 
     int set_option(Solution&, const std::string& k, const std::string& v) override {
-        if (k == "kernel") {
+        if (k == "block_steps") {
+            block_steps = std::max(1, atoi(v.c_str()));
+        } else if (k == "kernel") {
             if (v != "auto" && v != "tma" && v != "direct") return YB_EINVAL;
             kernel = v;
         } else if (k == "gen_sweep") {     // the generated engines' switch between their sweep and direct kernels
@@ -124,12 +153,29 @@ struct AvpEngine : Engine {
         else if (k == "gen_sweep") v = kernel == "direct" ? "0" : "1";
         else if (k == "lx") v = std::to_string(lx);
         else if (k == "grid") v = std::to_string(grid_override);
+        else if (k == "block_steps") v = std::to_string(block_steps);
+        else if (k == "tt_launches") v = std::to_string(tt_launches);
         else return false;
         return true;
     }
 
     template <class E>
     const AvpCfgT<E>& cfg() const { return *sweep_cfg<E>(shape, radius); }
+
+    // The temporal tile's storage on one rank: the spare pair of slots of A, and pads as deep as the tile's boxes of A(t) reach
+    // below the origin (2R rows / planes, 2 HZ columns), so that no TMA coordinate is negative.  Boxes that stick out at the upper
+    // end are zero-filled by the hardware, as in the one-step sweep.
+    void plan_storage(Solution& s) override {
+        Var& a = s.vars[0];
+        if (a.dev) return;
+        a.extra_slots = 0;
+        if (block_steps < 2 || kernel == "direct" || s.multi_rank() || !has_tt(s.spec)) return;
+        a.extra_slots = 2;
+        const int R = s.spec.radius, vw = 16 / s.spec.elem_bytes;
+        for (Dim& d : a.dims)
+            if (d.spec.kind == DIM_DOMAIN)
+                d.min_pad_l = std::max<int64_t>(d.min_pad_l, d.spec.domain_index == 2 ? 2 * ((R + vw - 1) / vw * vw) : 2 * R);
+    }
 
     int prepare(Solution& s) override {
         shape = avepts_shape(s.spec.name);
@@ -138,11 +184,14 @@ struct AvpEngine : Engine {
             return set_error(YB_EUNSUPPORTED, "%s: the hand-written sweep serves radius 1-%d", s.spec.name.c_str(), AVP_MAX_R);
         if (s.spec.elem_bytes != 4 && s.spec.elem_bytes != 8) return set_error(YB_EUNSUPPORTED, "%s: elements must be 4 or 8 bytes", s.spec.name.c_str());
         f64 = s.spec.elem_bytes == 8;
-        maps_ok = attr_set = false;
+        maps_ok = attr_set = tt_ok = false;
+        tt_launches = 0;
         cudaDeviceProp prop;
         YB_CUDA(cudaGetDeviceProperties(&prop, s.device));
+        num_sms = prop.multiProcessorCount;
+        if (s.vars[0].nslots() > 4) return set_error(YB_EUNSUPPORTED, "%s: at most 4 storage slots of A", s.spec.name.c_str());
         if (prop.major >= 9) {
-            if (int rc = f64 ? build<double>(s, prop.multiProcessorCount) : build<float>(s, prop.multiProcessorCount)) return rc;
+            if (int rc = f64 ? build<double>(s) : build<float>(s)) return rc;
             maps_ok = true;
         }
         preload_kernel(f64 ? (const void*)direct_fn<double>(shape) : (const void*)direct_fn<float>(shape));
@@ -150,16 +199,28 @@ struct AvpEngine : Engine {
     }
 
     template <class E>
-    int build(const Solution& s, int num_sms) {
+    int build(const Solution& s) {
         const AvpCfgT<E>& c = cfg<E>();
         const Var& a = s.vars[0];
-        for (int slot = 0; slot < 2; slot++)
+        const int nsl = a.nslots();
+        for (int slot = 0; slot < nsl; slot++)
             if (int rc = make_var_tensor_map(&maps[slot], a, slot, c.hp, c.hrows)) return rc;
         YB_CUDA(cudaFuncSetAttribute(c.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(c.smem)));
         int per_sm = 0;
         YB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, c.fn, c.threads, c.smem));
         gmax = std::max(1, per_sm) * num_sms;
         attr_set = true;
+        const AvpTTCfgT<E>* tc = tt_cfg<E>(shape, radius);
+        if (tc && a.extra_slots == 2 && nsl == 4) {
+            for (int slot = 0; slot < nsl; slot++)
+                if (int rc = make_var_tensor_map(&tt_maps[slot], a, slot, tc->ip, tc->irows)) return rc;
+            YB_CUDA(cudaFuncSetAttribute(tc->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(tc->smem)));
+            per_sm = 0;
+            YB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc->fn, tc->threads, tc->smem));
+            tt_gmax = std::max(1, per_sm) * num_sms;
+            preload_halo_shell_copy(int(sizeof(E)));
+            tt_ok = true;
+        }
         return 0;
     }
 
@@ -210,7 +271,62 @@ struct AvpEngine : Engine {
         return 1;
     }
 
-    // Offline tuner: the sweep's chunk length, timed over the whole rank box.  Every candidate computes the same bits.
+    // ---- temporal tile -------------------------------------------------------------------------------------------
+    int fused_steps(const Solution& s) const override {
+        return (tt_ok && block_steps >= 2 && kernel != "direct" && !s.multi_rank()) ? 2 : 1;
+    }
+
+    int begin_run(Solution& s, int64_t, cudaStream_t st) override { return copy_halo_shells(s.vars[0], num_sms, st); }
+
+    // Steps t+1 and t+2 in one sweep (avepts_tt2_kernel) over the whole rank domain: reads A(t) from the live pair of slots, writes
+    // A(t+2) into the partner of A(t)'s slot in the spare pair -- and A(t+1) into the partner of its slot when the launch ends the
+    // run -- then makes the spare pair the live one.
+    int launch_steps(Solution& s, int64_t t, int nsteps, bool ends_run, const Box& box, cudaStream_t st) override {
+        if (nsteps != 2 || !tt_ok) return set_error(YB_EUNSUPPORTED, "%s: no temporal tile for %d steps in this configuration", s.spec.name.c_str(), nsteps);
+        if (box.empty()) return 0;
+        for (int k = 0; k < 3; k++)
+            if (box.b[k] != 0 || box.e[k] != s.rank_size[k]) return set_error(YB_EUNSUPPORTED, "%s: the temporal tile runs on the whole rank domain", s.spec.name.c_str());
+        const int rc = f64 ? launch_tt<double>(s, t, ends_run, box, st) : launch_tt<float>(s, t, ends_run, box, st);
+        if (rc < 0) return rc;
+        tt_launches++;
+        s.vars[0].slot_bias ^= 2;       // steps t+1, t+2 (and every later access, stream-ordered) live in the other pair now
+        return 1;
+    }
+
+    template <class E>
+    int launch_tt(Solution& s, int64_t t, bool ends_run, const Box& box, cudaStream_t st) {
+        const AvpTTCfgT<E>& c = *tt_cfg<E>(shape, radius);
+        const Var& a = s.vars[0];
+        const Dim *dx = a.domain_dim(0), *dy = a.domain_dim(1), *dz = a.domain_dim(2);
+        const int cur = a.slot_of(t), nxt = a.slot_of(t + 1);         // nxt == cur ^ 1
+        auto at = [&](int slot) { return reinterpret_cast<E*>(a.slot_ptr(slot)) + a.origin_offset(); };
+        AvpTTParamsT<E> P{};
+        P.out = at(cur ^ 2);
+        P.cur = at(cur);
+        P.out1 = ends_run ? at(nxt ^ 2) : nullptr;
+        P.halo1 = at(nxt);
+        P.sx = dx->stride; P.sy = dy->stride;
+        P.x_begin = 0; P.x_end = int(box.e[0]);
+        P.y_begin = 0; P.y_end = int(box.e[1]);
+        P.z_begin = 0; P.z_end = int(box.e[2]);
+        P.pad_x = int(dx->pad_l); P.pad_y = int(dy->pad_l); P.pad_z = int(dz->pad_l);
+        P.scale = E(scale_of(shape, radius));
+        P.nty = int((box.e[1] + c.ty - 1) / c.ty);
+        P.ntz = int((box.e[2] + c.tz - 1) / c.tz);
+        const int64_t ntile = int64_t(P.nty) * P.ntz;
+        const int g = grid_override > 0 ? grid_override : tt_gmax;
+        const int64_t nx = box.e[0];
+        // a chunk loads 4R planes and computes 2R step-1 planes before its first result
+        P.nchunks = chunk_count(nx, ntile, g, lx, 4 * radius, 1, std::min<int64_t>(AVP_MAX_CHUNKS, nx));
+        chunk_partition(0, nx, P.nchunks, false, false, P.cx0, P.clen, nullptr);
+        const int grid = int(std::min<int64_t>(ntile * P.nchunks, g));
+        c.fn<<<grid, c.threads, c.smem, st>>>(tt_maps[cur], P);
+        YB_CUDA(cudaGetLastError());
+        return 1;
+    }
+
+    // Offline tuner: the sweep's chunk length, timed over the whole rank box; then, where the temporal tile is built, one step per
+    // sweep against two (block_steps), at that chunk length.  Every candidate computes the same bits.
     int auto_tune(Solution& s, cudaStream_t st, std::string& report) override {
         Box whole;
         for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = s.rank_size[d]; }
@@ -218,7 +334,7 @@ struct AvpEngine : Engine {
             report = s.spec.name + ": no tiled variants to tune for this configuration";
             return 0;
         }
-        const int keep_lx = lx;
+        const int keep_lx = lx, keep_bs = block_steps;
         int64_t t = s.vars[0].last_valid_step();
         double best_ms = 1e30;
         int best = 0;
@@ -229,12 +345,22 @@ struct AvpEngine : Engine {
             lx = l;
             const double ms = time_launches(st, 3, [&]() { return launch(s, 0, t++, whole, st); });
             if (ms < 0) { lx = keep_lx; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
-            snprintf(line, sizeof line, " lx=%d: %.4f ms/step\n", l, ms);
+            snprintf(line, sizeof line, " one step per sweep, lx=%d: %.4f ms/step\n", l, ms);
             report += line;
             if (ms < best_ms) { best_ms = ms; best = l; }
         }
         lx = best;
-        snprintf(line, sizeof line, "best: lx=%d (%.4f ms/step)\n", lx, best_ms);
+        if (tt_ok && !s.multi_rank()) {
+            if (int rc = begin_run(s, t, st)) return rc;
+            const double ms = time_launches(st, 3, [&]() { const int rc = launch_steps(s, t, 2, false, whole, st); t += 2; return rc; }) / 2;
+            if (ms < 0) { lx = keep_lx; block_steps = keep_bs; return set_error(YB_ECUDA, "auto-tuner: a trial launch failed"); }
+            snprintf(line, sizeof line, " two steps per sweep, lx=%d: %.4f ms/step\n", lx, ms);
+            report += line;
+            block_steps = ms < best_ms ? 2 : 1;
+            best_ms = std::min(best_ms, ms);
+            s.options["block_steps"] = std::to_string(block_steps);
+        }
+        snprintf(line, sizeof line, "best: lx=%d block_steps=%d (%.4f ms/step)\n", lx, block_steps, best_ms);
         report += line;
         s.options["lx"] = std::to_string(lx);
         return 0;

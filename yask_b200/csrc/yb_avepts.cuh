@@ -154,6 +154,62 @@ __device__ __forceinline__ void avp_load_point(const uint8_t* p, int dz, typenam
     }
 }
 
+// The sum, in the reference's order, of the points of one 16-byte vector staged in shared memory: pl[R + dx] is the vector in the
+// plane dx away (dx = -R..R), plane(dx) the same for a run-time dx, and rows are ROWB bytes apart.  acc comes back unscaled.
+template <class T, int ROWB, class PF>
+__device__ __forceinline__ void avp_sum(const uint8_t* const* pl, PF&& plane, typename T::E (&acc)[T::VW]) {
+    using E = typename T::E;
+    using V = typename T::V;
+    constexpr int R = T::R, VW = T::VW, ES = T::ES, HZ = T::HZ;
+    avp_load_point<T>(pl[R], 0, acc);
+    avp_star_points<T::SHAPE>(
+        R,
+        [&](int dx, int dy, int dz) {
+            E v[VW];
+            avp_load_point<T>(pl[R + dx] + dy * ROWB, dz, v);
+#pragma unroll
+            for (int i = 0; i < VW; i++) acc[i] = acc[i] + v[i];
+        },
+        [&](int dx, int dy, int dz) {       // run-time offsets: one scalar load per element
+            const E* v = reinterpret_cast<const E*>(plane(dx) + dy * ROWB) + dz;
+#pragma unroll
+            for (int i = 0; i < VW; i++) acc[i] = acc[i] + v[i];
+        });
+    if constexpr (T::SHAPE == AVP_CUBE) {
+        constexpr int WN = VW + 2 * HZ;
+#pragma unroll 1
+        for (int rx = 1; rx <= R; rx++) {
+#pragma unroll 1
+            for (int ry = 1; ry <= R; ry++) {
+                // rows (rx, ry), (rx, -ry), (-rx, ry), (-rx, -ry) over the z window [-HZ, VW + HZ)
+                E w[4][WN];
+                const uint8_t *px = plane(rx), *mx = plane(-rx);
+                const uint8_t* ro[4] = {px + ry * ROWB, px - ry * ROWB, mx + ry * ROWB, mx - ry * ROWB};
+#pragma unroll
+                for (int k = 0; k < 4; k++)
+#pragma unroll
+                    for (int c = 0; c < WN / VW; c++)
+                        f4_to_arr(*reinterpret_cast<const V*>(ro[k] + (c * VW - HZ) * ES), &w[k][c * VW]);
+#pragma unroll
+                for (int rz = 1; rz <= R; rz++)
+#pragma unroll
+                    for (int i = 0; i < VW; i++) {
+                        E a = acc[i];
+                        a = a + w[0][HZ + i + rz];      // ( rx,  ry,  rz)
+                        a = a + w[1][HZ + i - rz];      // ( rx, -ry, -rz)
+                        a = a + w[0][HZ + i - rz];      // ( rx,  ry, -rz)
+                        a = a + w[1][HZ + i + rz];      // ( rx, -ry,  rz)
+                        a = a + w[2][HZ + i + rz];      // (-rx,  ry,  rz)
+                        a = a + w[3][HZ + i - rz];      // (-rx, -ry, -rz)
+                        a = a + w[2][HZ + i - rz];      // (-rx,  ry, -rz)
+                        a = a + w[3][HZ + i + rz];      // (-rx, -ry,  rz)
+                        acc[i] = a;
+                    }
+            }
+        }
+    }
+}
+
 template <class T>
 __global__ void __launch_bounds__(T::THREADS + 32, 1)
 avepts_sweep_kernel(const __grid_constant__ CUtensorMap M, const __grid_constant__ AvpParamsT<typename T::E> P) {
@@ -228,53 +284,7 @@ avepts_sweep_kernel(const __grid_constant__ CUtensorMap M, const __grid_constant
             // the same for a run-time dx (an index into pl[] would put it in local memory)
             auto plane = [&](int dx) { return sbase + ((gc + dx) % NS) * T::SLOT_BYTES + own; };
             E acc[VW];
-            avp_load_point<T>(pl[R], 0, acc);
-            avp_star_points<T::SHAPE>(
-                R,
-                [&](int dx, int dy, int dz) {
-                    E v[VW];
-                    avp_load_point<T>(pl[R + dx] + dy * (HP * ES), dz, v);
-#pragma unroll
-                    for (int i = 0; i < VW; i++) acc[i] = acc[i] + v[i];
-                },
-                [&](int dx, int dy, int dz) {       // run-time offsets: one scalar load per element
-                    const E* v = reinterpret_cast<const E*>(plane(dx) + dy * (HP * ES)) + dz;
-#pragma unroll
-                    for (int i = 0; i < VW; i++) acc[i] = acc[i] + v[i];
-                });
-            if constexpr (T::SHAPE == AVP_CUBE) {
-                constexpr int WN = VW + 2 * HZ;
-#pragma unroll 1
-                for (int rx = 1; rx <= R; rx++) {
-#pragma unroll 1
-                    for (int ry = 1; ry <= R; ry++) {
-                        // rows (rx, ry), (rx, -ry), (-rx, ry), (-rx, -ry) over the z window [-HZ, VW + HZ)
-                        E w[4][WN];
-                        const uint8_t *px = plane(rx), *mx = plane(-rx);
-                        const uint8_t* ro[4] = {px + ry * (HP * ES), px - ry * (HP * ES), mx + ry * (HP * ES), mx - ry * (HP * ES)};
-#pragma unroll
-                        for (int k = 0; k < 4; k++)
-#pragma unroll
-                            for (int c = 0; c < WN / VW; c++)
-                                f4_to_arr(*reinterpret_cast<const V*>(ro[k] + (c * VW - HZ) * ES), &w[k][c * VW]);
-#pragma unroll
-                        for (int rz = 1; rz <= R; rz++)
-#pragma unroll
-                            for (int i = 0; i < VW; i++) {
-                                E a = acc[i];
-                                a = a + w[0][HZ + i + rz];      // ( rx,  ry,  rz)
-                                a = a + w[1][HZ + i - rz];      // ( rx, -ry, -rz)
-                                a = a + w[0][HZ + i - rz];      // ( rx,  ry, -rz)
-                                a = a + w[1][HZ + i + rz];      // ( rx, -ry,  rz)
-                                a = a + w[2][HZ + i + rz];      // (-rx,  ry,  rz)
-                                a = a + w[3][HZ + i - rz];      // (-rx, -ry, -rz)
-                                a = a + w[2][HZ + i - rz];      // (-rx,  ry, -rz)
-                                a = a + w[3][HZ + i + rz];      // (-rx, -ry,  rz)
-                                acc[i] = a;
-                            }
-                    }
-                }
-            }
+            avp_sum<T, HP * ES>(pl, plane, acc);
             E res[VW];
 #pragma unroll
             for (int i = 0; i < VW; i++) res[i] = acc[i] * P.scale;

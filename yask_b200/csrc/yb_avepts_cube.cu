@@ -3,4 +3,5 @@
 
 namespace yb {
 YB_AVP_TABLES(AVP_CUBE)
+YB_AVP_TT_TABLES(AVP_CUBE, 0, 0)     // no temporal tile: slower with pairs on an H100 (README)
 }  // namespace yb

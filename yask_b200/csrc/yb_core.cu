@@ -830,7 +830,8 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled)) ? s->engine->fused_steps(*s) : 1;
     if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
-        rc = s->halo ? halo_run_steps(*s, t_first, fs, st) : s->engine->launch_steps(*s, t_first, fs, whole, st);
+        const bool ends_run = t_first + fs - 1 == last_step;
+        rc = s->halo ? halo_run_steps(*s, t_first, fs, st) : s->engine->launch_steps(*s, t_first, fs, ends_run, whole, st);
         if (rc < 0) break;
         s->stats.kernel_launches += rc;
         for (int k = 0; k < fs; k++) {

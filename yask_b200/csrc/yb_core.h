@@ -163,8 +163,10 @@ struct Engine {
     virtual int fused_steps(const Solution&) const { return 1; }
     // called once per run_solution() before the first step (first_step = t of the first launch)
     virtual int begin_run(Solution&, int64_t /*first_step*/, cudaStream_t) { return 0; }
-    // all stages of steps t+1 .. t+nsteps in one go; returns #kernels launched or <0
-    virtual int launch_steps(Solution&, int64_t /*t*/, int /*nsteps*/, const Box&, cudaStream_t) { return YB_EUNSUPPORTED; }
+    // all stages of steps t+1 .. t+nsteps in one go; returns #kernels launched or <0.  ends_run: step t+nsteps is the last of the
+    // run_solution() call, so every step of the API's window must be stored; otherwise an engine may skip storing a step that no
+    // later launch reads (the average-of-points tile keeps A(t+1) in shared memory).
+    virtual int launch_steps(Solution&, int64_t /*t*/, int /*nsteps*/, bool /*ends_run*/, const Box&, cudaStream_t) { return YB_EUNSUPPORTED; }
 };
 
 struct HaloState;  // yb_halo.cu
@@ -279,6 +281,12 @@ int registry_create(const std::string& name, int radius, int elem_bytes, Stencil
 // CUtensorMap (passed as void* to keep <cuda.h> out of this header) over one step slot of a full-rank 3-D var,
 // box (box_z, box_y, 1) -- yb_iso3dfd.cu
 int make_var_tensor_map(void* map, const Var& v, int slot, int box_z, int box_y);
+
+// Temporal tiles (Var::extra_slots == 2): copy the halo cells of the live pair of slots of `v` into the spare pair, so that the
+// pair a fused launch writes holds the halo cells the reference's two slots would -- yb_iso3dfd.cu.  The copy kernel is loaded by
+// preload_halo_shell_copy().
+int copy_halo_shells(const Var& v, int num_sms, cudaStream_t st);
+void preload_halo_shell_copy(int elem_bytes);
 
 // engines
 std::unique_ptr<Engine> make_iso3dfd_engine();

@@ -460,7 +460,8 @@ int halo_run_steps(Solution& s, int64_t t, int nsteps, cudaStream_t st) {
     if (int rc = halo_flush_wait(s, st)) return rc;
     Box whole;
     for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = d < s.ndd ? s.rank_size[d] : 1; }
-    const int rc = s.engine->launch_steps(s, t, nsteps, whole, st);
+    // the deep exchange below sends both newest steps, so every fused launch stores them (ends_run)
+    const int rc = s.engine->launch_steps(s, t, nsteps, true, whole, st);
     if (rc < 0) return rc;
     for (const StageSpec& sp : s.spec.stages)
         for (int vi : sp.outputs)

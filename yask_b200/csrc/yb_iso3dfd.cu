@@ -273,7 +273,8 @@ DirectFn<E> direct_kernel(bool sponge, int mode) {
 // Copies a box of cells from one step slot to another (same geometry): keeps the halo cells of the extra storage
 // slots of a temporally tiled var equal to those of the slot two steps earlier -- what the reference's two-slot storage
 // gives by construction (p(t+2) lives in the memory of p(t), halo cells included).
-__global__ void slot_box_copy_kernel(float* dst, const float* src, long long sx, long long sy, int bx, int by, int bz, int ex, int ey, int ez) {
+template <class T>      // T: an unsigned integer of the element size (the copy moves bits)
+__global__ void slot_box_copy_kernel(T* dst, const T* src, long long sx, long long sy, int bx, int by, int bz, int ex, int ey, int ez) {
     const long long n = (long long)ex * ey * ez;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int z = int(i % ez);
@@ -283,6 +284,48 @@ __global__ void slot_box_copy_kernel(float* dst, const float* src, long long sx,
         dst[o] = src[o];
     }
 }
+
+}  // namespace
+
+// Halo cells of the spare pair of slots take those of the live pair, so that whichever pair a fused launch reads holds the halo
+// cells the reference's two slots would (kernels never write halo cells; the API may, between runs).
+int copy_halo_shells(const Var& v, int num_sms, cudaStream_t st) {
+    if (v.extra_slots != 2 || !v.dev) return 0;
+    const Dim* d[3] = {v.domain_dim(0), v.domain_dim(1), v.domain_dim(2)};
+    int64_t lo[3], hi[3], db[3], de[3];     // halo box and domain box in alloc coordinates
+    for (int k = 0; k < 3; k++) {
+        db[k] = d[k]->pad_l; de[k] = d[k]->pad_l + d[k]->domain;
+        lo[k] = db[k] - d[k]->spec.halo_l; hi[k] = de[k] + d[k]->spec.halo_r;
+    }
+    for (int pair = 0; pair < 2; pair++) {
+        const void* src = v.slot_ptr(v.slot_bias + pair);
+        void* dst = v.slot_ptr((v.slot_bias ^ 2) + pair);
+        // shell = x slabs over the whole (y,z) halo box, y slabs over the domain's x range, z slabs over the domain's x and y ranges
+        const int64_t slabs[6][6] = {{lo[0], db[0], lo[1], hi[1], lo[2], hi[2]}, {de[0], hi[0], lo[1], hi[1], lo[2], hi[2]},
+                                     {db[0], de[0], lo[1], db[1], lo[2], hi[2]}, {db[0], de[0], de[1], hi[1], lo[2], hi[2]},
+                                     {db[0], de[0], db[1], de[1], lo[2], db[2]}, {db[0], de[0], db[1], de[1], de[2], hi[2]}};
+        for (auto& b : slabs) {
+            const int64_t ex = b[1] - b[0], ey = b[3] - b[2], ez = b[5] - b[4];
+            if (ex <= 0 || ey <= 0 || ez <= 0) continue;
+            const int64_t n = ex * ey * ez;
+            const int grid = int(std::min<int64_t>((n + 255) / 256, 16 * num_sms));
+            if (v.elem_bytes == 8)
+                slot_box_copy_kernel<<<grid, 256, 0, st>>>(static_cast<uint64_t*>(dst), static_cast<const uint64_t*>(src), d[0]->stride,
+                                                           d[1]->stride, int(b[0]), int(b[2]), int(b[4]), int(ex), int(ey), int(ez));
+            else
+                slot_box_copy_kernel<<<grid, 256, 0, st>>>(static_cast<uint32_t*>(dst), static_cast<const uint32_t*>(src), d[0]->stride,
+                                                           d[1]->stride, int(b[0]), int(b[2]), int(b[4]), int(ex), int(ey), int(ez));
+        }
+    }
+    YB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+void preload_halo_shell_copy(int elem_bytes) {
+    preload_kernel(elem_bytes == 8 ? (const void*)slot_box_copy_kernel<uint64_t> : (const void*)slot_box_copy_kernel<uint32_t>);
+}
+
+namespace {
 
 struct IsoEngine : Engine {
     int radius = 8;
@@ -453,7 +496,7 @@ struct IsoEngine : Engine {
                     tts.push_back(w);
                 }
                 tt_ok = true;
-                preload_kernel((const void*)slot_box_copy_kernel);
+                preload_halo_shell_copy(4);
             }
         }
         for (int m = 0; m < 3; m++)
@@ -616,39 +659,12 @@ struct IsoEngine : Engine {
         return (tt_ok && block_steps >= 2 && kernel != "direct") ? 2 : 1;
     }
 
-    // Halo cells of the spare pair of slots take those of the live pair, so that whichever pair a fused launch reads holds
-    // the halo cells the reference's two slots would (kernels never write halo cells; the API may, between runs).
-    int begin_run(Solution& s, int64_t, cudaStream_t st) override {
-        const Var& p = s.vars[0];
-        if (p.extra_slots != 2 || !p.dev) return 0;
-        const Dim* d[3] = {p.domain_dim(0), p.domain_dim(1), p.domain_dim(2)};
-        int64_t lo[3], hi[3], db[3], de[3];     // halo box and domain box in alloc coordinates
-        for (int k = 0; k < 3; k++) {
-            db[k] = d[k]->pad_l; de[k] = d[k]->pad_l + d[k]->domain;
-            lo[k] = db[k] - d[k]->spec.halo_l; hi[k] = de[k] + d[k]->spec.halo_r;
-        }
-        for (int pair = 0; pair < 2; pair++) {
-            const float* src = reinterpret_cast<const float*>(p.slot_ptr(p.slot_bias + pair));
-            float* dst = reinterpret_cast<float*>(p.slot_ptr((p.slot_bias ^ 2) + pair));
-            // shell = x slabs over the whole (y,z) halo box, y slabs over the domain's x range, z slabs over the domain's x and y ranges
-            const int64_t slabs[6][6] = {{lo[0], db[0], lo[1], hi[1], lo[2], hi[2]}, {de[0], hi[0], lo[1], hi[1], lo[2], hi[2]},
-                                         {db[0], de[0], lo[1], db[1], lo[2], hi[2]}, {db[0], de[0], de[1], hi[1], lo[2], hi[2]},
-                                         {db[0], de[0], db[1], de[1], lo[2], db[2]}, {db[0], de[0], db[1], de[1], de[2], hi[2]}};
-            for (auto& b : slabs) {
-                const int64_t ex = b[1] - b[0], ey = b[3] - b[2], ez = b[5] - b[4];
-                if (ex <= 0 || ey <= 0 || ez <= 0) continue;
-                const int64_t n = ex * ey * ez;
-                const int grid = int(std::min<int64_t>((n + 255) / 256, 16 * num_sms));
-                slot_box_copy_kernel<<<grid, 256, 0, st>>>(dst, src, d[0]->stride, d[1]->stride, int(b[0]), int(b[2]), int(b[4]), int(ex), int(ey), int(ez));
-            }
-        }
-        YB_CUDA(cudaGetLastError());
-        return 0;
-    }
+    int begin_run(Solution& s, int64_t, cudaStream_t st) override { return copy_halo_shells(s.vars[0], num_sms, st); }
 
     // Steps t+1 and t+2 in one sweep (iso3dfd_tt2_kernel): reads the live pair of slots (p(t-1), p(t)), writes p(t+1) / p(t+2)
-    // into the partners of p(t-1) / p(t) in the spare pair, which then becomes the live one.
-    int launch_steps(Solution& s, int64_t t, int nsteps, const Box& box, cudaStream_t st) override {
+    // into the partners of p(t-1) / p(t) in the spare pair, which then becomes the live one.  Both steps are always stored
+    // (ends_run is not needed): step t+3 reads p(t+1).
+    int launch_steps(Solution& s, int64_t t, int nsteps, bool, const Box& box, cudaStream_t st) override {
         if (nsteps != 2 || !tt_ok) return set_error(YB_EUNSUPPORTED, "iso3dfd: no temporal tile for %d steps in this configuration", nsteps);
         if (box.empty()) return 0;
         SweepForm<TTCfg, TTMaps>& w = tts[tt_var()];
@@ -745,7 +761,7 @@ struct IsoEngine : Engine {
                     return ms;
                 }
                 tt_variant = cand - 1;
-                const double ms = time_launches(st, 3, [&]() { const int rc = launch_steps(s, t, 2, whole, st); t += 2; return rc; }) / 2;
+                const double ms = time_launches(st, 3, [&]() { const int rc = launch_steps(s, t, 2, false, whole, st); t += 2; return rc; }) / 2;
                 snprintf(line, sizeof line, " two steps per sweep, %s: %.4f ms/step\n", tts[tt_variant].cfg->name, ms);
                 return ms;
             }))

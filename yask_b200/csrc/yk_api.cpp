@@ -643,7 +643,8 @@ struct B200Solution : yk_solution {
         return " -g<dim> <n>   overall domain size        -l<dim> <n>   rank domain size\n"
                " -nr<dim> <n>  ranks in dim               -ri<dim> <n>  rank index in dim\n"
                " -mp<dim> <n>  minimum padding            -b<dim> <n>   block size (recorded; no effect on the GPU)\n"
-               " -bt <n>       block steps: n >= 2 selects the temporal tile where the engine has one (iso3dfd radius <= 2)\n"
+               " -bt <n>       block steps: n >= 2 selects the temporal tile where the engine has one (iso3dfd fp32 radius <= 2;\n"
+               "               3axis radius <= 2 in fp32 and fp64 on one rank)\n"
                " -Mbt <n>      mega-block steps: with -bt 2, n >= 2 runs the temporal tile on rank grids too, halos exchanged once per 2 steps\n"
                " -fp_mode 0|1|2  FP contraction mode      -kernel auto|tma|direct   -tile <n>   -lx <n>   -device <n>\n";
     }
