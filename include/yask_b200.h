@@ -208,6 +208,28 @@ int yb_solution_sync(yb_solution* s);              /* wait for all queued device
 int yb_get_stats(yb_solution* s, yb_stats* out);   /* get_stats (syncs) */
 int yb_clear_stats(yb_solution* s);                /* clear_stats */
 
+/* ---- point sources and receivers, applied on the device inside run_solution() ------------------------------------
+ * Replaces the host loop run_solution(t, t); add_to_element(amp[t], {t+1, src}); get_element({t+1, rcv}) with one call.
+ * Whenever a run has computed step u (after all its stages; u = t+1, or t-1 for a reverse solution):
+ *   1. if 0 <= u - t0 < nrows: var(u, idx_i) += amp[u - t0][i] for every source i in list order, rounded as add_to_element
+ *      (fp32: float(float(old) + float(amp)); fp64: old + amp);
+ *   2. then, if 0 <= u - t0r < nrows_r: trace[u - t0r][j] = var(u, ridx_j) in the element type.
+ * `idx` holds n (m) points of num_domain_dims GLOBAL domain indices each, row-major; every index must lie in the overall
+ * domain (halo and pad cells are refused).  The var must have the step dim and every domain dim, no misc dim, and be written
+ * by a stage; on a rank grid a source var must be written by the last stage.  The sets persist across runs until cleared or
+ * replaced; a rank keeps only the points of its own domain.  Legal before or after prepare (checked as soon as the rank
+ * geometry is known; a prepared solution synchronizes its stream and uploads the tables).  While points are set every run takes
+ * one step per launch (block_steps pairs resume once they are cleared); a rank grid whose halos are exchanged once per pair of
+ * steps (block_steps=2 + mega_block_steps=2) refuses them.  Read-only option point_launches: point-kernel launches since prepare. */
+int yb_solution_set_sources(yb_solution* s, const char* var, int64_t n, const int64_t* idx, int64_t t0, int64_t nrows,
+                            const double* amp /* nrows x n */);
+int yb_solution_set_receivers(yb_solution* s, const char* var, int64_t m, const int64_t* idx, int64_t t0r, int64_t nrows_r);
+/* Copy the traces (nrows_r x m elements of the solution's type; rows not recorded yet are 0) into `out` and set owned[j] = 1
+ * for the receivers this rank records (0 for the others, whose columns stay 0).  `out` may be NULL: then only the mask, which
+ * needs no device once the rank geometry is known (plan_geometry). */
+int yb_solution_get_traces(yb_solution* s, void* out, uint8_t* owned);
+int yb_solution_clear_points(yb_solution* s);      /* remove both sets */
+
 /* ---- multi-GPU halo exchange, one process per GPU (replaces exchange_halos, halo.cpp:80-491) --- */
 /* Each rank exports an opaque blob (CUDA IPC handles of its var storage + sync flags), the
  * launcher all-gathers the blobs (torch.distributed / MPI / files) and imports every

@@ -60,7 +60,8 @@ ABI_SYMBOLS = [
     "yb_solution_plan_geometry", "yb_solution_prepare", "yb_solution_is_prepared", "yb_num_vars", "yb_var_index", "yb_var_info_get", "yb_var_create", "yb_var_fuse", "yb_var_set_min_pad",
     "yb_var_set_slice", "yb_var_get_slice", "yb_var_set_slice_device", "yb_var_get_slice_device", "yb_var_set_all_same",
     "yb_var_set_slice_same", "yb_var_reduce_slice", "yb_solution_auto_tune", "yb_solution_reset_auto_tuner", "yb_solution_is_auto_tuner_enabled", "yb_solution_auto_tuner_report", "yb_var_fill_hash", "yb_var_fill_hash_shifted", "yb_var_checksum", "yb_var_device_ptr", "yb_copy_to_host", "yb_solution_run", "yb_solution_sync",
-    "yb_get_stats", "yb_clear_stats", "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
+    "yb_get_stats", "yb_clear_stats", "yb_solution_set_sources", "yb_solution_set_receivers", "yb_solution_get_traces",
+    "yb_solution_clear_points", "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
 ]
@@ -125,6 +126,10 @@ def lib() -> C.CDLL:
         L.yb_solution_sync.argtypes = [p]
         L.yb_get_stats.argtypes = [p, C.POINTER(Stats)]
         L.yb_clear_stats.argtypes = [p]
+        L.yb_solution_set_sources.argtypes = [p, C.c_char_p, i64, C.POINTER(i64), i64, i64, C.POINTER(C.c_double)]
+        L.yb_solution_set_receivers.argtypes = [p, C.c_char_p, i64, C.POINTER(i64), i64, i64]
+        L.yb_solution_get_traces.argtypes = [p, p, C.POINTER(C.c_uint8)]
+        L.yb_solution_clear_points.argtypes = [p]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
         L.yb_halo_export.argtypes = [p, p, C.c_size_t]
         L.yb_halo_import.argtypes = [p, i64, p, C.c_size_t]
@@ -393,6 +398,53 @@ class Solution:
 
     def clear_stats(self):
         _chk(lib().yb_clear_stats(self._h))
+
+    # point sources and receivers (yb_solution_set_sources / set_receivers / get_traces / clear_points)
+    def _points(self, idx, what: str) -> np.ndarray:
+        nd = len(self.get_domain_dim_names())
+        a = np.asarray(idx, dtype=np.int64)
+        if a.ndim == 1 and nd == 1:
+            a = a.reshape(-1, 1)
+        if a.ndim != 2 or a.shape[1] != nd or a.shape[0] < 1:
+            raise YaskError(-1, f"{what}: expected a list of points with {nd} domain index(es) each "
+                                f"({', '.join(self.get_domain_dim_names())}), got shape {a.shape}")
+        return np.ascontiguousarray(a)
+
+    def set_sources(self, var: str, idx, t0: int, amp):
+        """Add amp[u - t0][i] to var(u, idx[i]) (list order, element-type rounding) after every step u a run computes with
+        0 <= u - t0 < len(amp).  idx: N points of global domain indices; amp: (nrows, N)."""
+        pts = self._points(idx, "sources")
+        a = np.asarray(amp, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != pts.shape[0]:
+            raise YaskError(-1, f"sources: amplitude table of shape {a.shape} does not match {pts.shape[0]} source point(s): "
+                                f"expected (nrows, {pts.shape[0]})")
+        a = np.ascontiguousarray(a)
+        _chk(lib().yb_solution_set_sources(self._h, var.encode(), pts.shape[0], pts.ctypes.data_as(C.POINTER(C.c_int64)),
+                                           int(t0), a.shape[0], a.ctypes.data_as(C.POINTER(C.c_double))))
+
+    def set_receivers(self, var: str, idx, t0: int, nrows: int):
+        """Record var(u, idx[j]) into trace row u - t0 after every step u a run computes with 0 <= u - t0 < nrows."""
+        pts = self._points(idx, "receivers")
+        _chk(lib().yb_solution_set_receivers(self._h, var.encode(), pts.shape[0], pts.ctypes.data_as(C.POINTER(C.c_int64)),
+                                             int(t0), int(nrows)))
+        self._nrcv, self._nrows_r = pts.shape[0], int(nrows)
+
+    def get_traces(self):
+        """(traces, owned): traces (nrows, M) in the element dtype, owned[j] True for the receivers this rank records."""
+        dt = np.float32 if self.get_element_bytes() == 4 else np.float64
+        m, nrows = getattr(self, "_nrcv", 0), getattr(self, "_nrows_r", 0)
+        out = np.zeros((nrows, m), dtype=dt)
+        owned = np.zeros(m, dtype=np.uint8)
+        _chk(lib().yb_solution_get_traces(self._h, out.ctypes.data if self.is_prepared() else None,
+                                          owned.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return out, owned.astype(bool)
+
+    def clear_points(self):
+        _chk(lib().yb_solution_clear_points(self._h))
+        self._nrcv = self._nrows_r = 0
+
+    def is_prepared(self) -> bool:
+        return bool(lib().yb_solution_is_prepared(self._h))
 
     # multi-GPU plumbing (yb_halo_*)
     def halo_export(self) -> bytes:

@@ -11,6 +11,7 @@
 
 #include "yb_core.h"
 #include "yb_halo.h"
+#include "yb_points.h"
 
 namespace yb {
 
@@ -39,6 +40,7 @@ Solution::~Solution() {
         if (own_stream) cudaStreamDestroy(own_stream);
         if (comm_stream) cudaStreamDestroy(comm_stream);
     }
+    points_free(points);     // device tables are released on `device`, selected above
 }
 
 static int check_dim(const Solution* s, int dim) {
@@ -380,6 +382,8 @@ int yb_set_option(yb_solution* s_, const char* key, const char* value) {
     } else if (k == "auto_tune") {
         s->tuner = Solution::InRunTuner();
         s->tuner.enabled = atoi(value) != 0;
+    } else if (k == "point_launches" || k == "point_groups") {
+        return set_error(YB_EINVAL, "option '%s' is read-only", key);
     } else if (k == "overlap_comms" || k == "min_exterior" || k == "fused_halo" || k == "dma_halo") {
         // consumed by the halo engine at run time
     } else if (s->engine->set_option(*s, k, v) != 0) {
@@ -393,6 +397,8 @@ int yb_get_option(const yb_solution* s_, const char* key, char* value, size_t n)
     if (!s || !key || !value || !n) return set_error(YB_EINVAL, "null argument");
     std::string v;
     if (std::string(key) == "fp_mode") v = std::to_string(s->fp_mode);
+    else if (std::string(key) == "point_launches") v = std::to_string(s->points ? s->points->launches : 0);   // read-only
+    else if (std::string(key) == "point_groups") v = points_groups_text(*s);                                    // read-only
     else if (!s->engine->get_option(*s, key, v)) {
         auto it = s->options.find(key);
         if (it == s->options.end()) return set_error(YB_EINVAL, "unknown option '%s'", key);
@@ -423,7 +429,9 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     if (int rc = compute_rank_geometry(*s)) return rc;
     plan_storage(*s);
     for (auto& v : s->vars) compute_var_geometry(*s, v);
-    return s->engine->check_geometry(*s);
+    s->geometry_planned = true;
+    if (int rc = s->engine->check_geometry(*s)) return rc;
+    return points_active(*s) ? points_plan(*s) : 0;      // point sets given before the geometry are checked now
 }
 
 int yb_solution_prepare(yb_solution* s_, int device) {
@@ -434,6 +442,7 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (ndev <= 0) return set_error(YB_ECUDA, "no CUDA device available: the yask_b200 engine has no CPU fallback");
     if (device < 0 || device >= ndev) return set_error(YB_EINVAL, "device %d out of range [0,%d)", device, ndev);
     if (int rc = compute_rank_geometry(*s)) return rc;
+    s->geometry_planned = true;
     plan_storage(*s);
     // a size the kernels cannot address is refused before any storage is allocated
     for (auto& v : s->vars)
@@ -459,12 +468,19 @@ int yb_solution_prepare(yb_solution* s_, int device) {
         YB_CUDA(cudaMemsetAsync(v.dev, 0, v.bytes(), s->stream()));
     }
     if (int rc = s->engine->prepare(*s)) return rc;
+    points_preload();
     if (s->multi_rank()) {
         if (int rc = halo_prepare(*s)) return rc;
     }
     YB_CUDA(cudaStreamSynchronize(s->stream()));
     s->prepared = true;
     memset(&s->stats, 0, sizeof s->stats);
+    if (s->points) {
+        // the point tables follow the final geometry; a set this geometry refuses is reported by the first run
+        s->points->stale = true;
+        s->points->launches = 0;
+        if (points_begin_run(*s) == YB_ECUDA) return YB_ECUDA;
+    }
     return 0;
 }
 int yb_solution_is_prepared(const yb_solution* s) { return s && CSOL(s)->prepared; }
@@ -792,6 +808,8 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     if (!s->prepared) return set_error(YB_ESTATE, "run_solution() called without calling prepare_solution() first");
     YB_CUDA(cudaSetDevice(s->device));
     cudaStream_t st = s->stream();
+    // point tables are normally uploaded when they are set (or at prepare); before anything of this run is enqueued otherwise
+    if (int rc = points_begin_run(*s)) return rc;
     // Timing events: pairs of finished runs are folded into the stats and recycled here, so that calling
     // run_solution(t) once per step (the reference's usual pattern) keeps a bounded number of events alive.
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -825,9 +843,11 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     if (rc >= 0) rc = s->engine->begin_run(*s, first_step, st);
     // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward run goes through the engine's fused launch, `fs` steps
     // at a time; what is left over (and every other kind of run) takes the one-step path below.  A rank grid fuses steps only
-    // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.
+    // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.  Point sources
+    // enter between two steps, so a solution with points runs one step per launch (points_check_mode refuses them on a rank
+    // grid in the fused mode).
     int64_t t_first = first_step;
-    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled)) ? s->engine->fused_steps(*s) : 1;
+    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s)) ? s->engine->fused_steps(*s) : 1;
     if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
         const bool ends_run = t_first + fs - 1 == last_step;
@@ -873,6 +893,8 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
             s->stats.est_fp_ops_done += sp.fp_ops * pts;
             for (int vi : sp.outputs) s->vars[vi].update_valid_step(t + sp.out_step_off);
         }
+        // sources and receivers of the step just computed (a rank grid applies them inside its last stage, halo_run_stage)
+        if (rc >= 0 && !s->halo) rc = points_launch(*s, t, PTS_ALL, whole, st);
         s->stats.num_steps_done++;
         if (tv >= 0 && te0 && te1) {
             cudaEventRecord(te1, st);

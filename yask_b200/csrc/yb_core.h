@@ -171,6 +171,8 @@ struct Engine {
 
 struct HaloState;  // yb_halo.cu
 void halo_free(HaloState*);
+struct PointsState;  // yb_points.cu
+void points_free(PointsState*);
 
 struct Solution {
     StencilSpec spec;
@@ -189,6 +191,7 @@ struct Solution {
     std::vector<Var> vars;
     std::map<std::string, std::string> options;
     int fp_mode = YB_FP_REF_GCC;
+    bool geometry_planned = false;   // plan_geometry() has derived the rank geometry (prepare() does too)
     bool prepared = false;
     int device = -1;
     cudaStream_t own_stream = nullptr, user_stream = nullptr, comm_stream = nullptr;
@@ -212,6 +215,8 @@ struct Solution {
     size_t stage_host_bytes = 0;
     // multi-GPU
     HaloState* halo = nullptr;   // owned; freed by halo_free()
+    // point sources and receivers (yb_points.h)
+    PointsState* points = nullptr;   // owned; freed by points_free()
     // Fused halo stores (set by the halo layer before a stage launch, consumed by an engine that can store its
     // boundary planes straight into the x neighbours' halo cells): element (0,0,0)-relative base pointers of the
     // OUTPUT var's step slot in the lower / upper x neighbour, or null.  The engine sets `used` if it honoured them.

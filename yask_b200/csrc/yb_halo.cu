@@ -24,6 +24,7 @@
 #include <cuda.h>
 
 #include "yb_halo.h"
+#include "yb_points.h"
 
 namespace yb {
 
@@ -487,6 +488,12 @@ static bool other_dirty(const HaloState* h, int var, int slot) {
 //     stores them into the neighbours' HBM as it computes them and publishes the epoch itself (IsoParams::sig_*);
 //   * split: one launch per exterior slab, push kernels + epoch publication, then the interior launch;
 //   * whole (domain too thin to split, stages with scratch vars, option overlap_comms=0): whole box, then push.
+// Point sources and receivers (yb_points.h) are applied in the last stage of the step, and a source is in its slot before the
+// exchange that publishes it: split form -- exterior points after the exterior launches, before the pushes and signals; the others
+// after the interior launch; whole form -- after the launch, before the push; fused form -- after the launch, for sources farther
+// than the widest x halo from every x interface (no neighbour reads them).  A rank that owns a source nearer than that runs the
+// stage in the split form instead: the fused launch stores and publishes its boundary planes itself, before a source could enter.
+// Both forms advance the epoch once, so the choice is the rank's own.
 int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     Box whole;
     for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = d < s.ndd ? s.rank_size[d] : 1; }
@@ -499,13 +506,19 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     };
     auto opt_off = [&](const char* key) { auto it = s.options.find(key); return it != s.options.end() && it->second == "0"; };
     const bool overlap = !opt_off("overlap_comms");
+    const bool points = stage + 1 == int(s.spec.stages.size()) && points_active(s);
+    auto apply_points = [&](int sel, const Box& interior) { return points ? points_launch(s, t, sel, interior, st) : 0; };
+    int64_t wx = 0;         // widest x halo: the planes of an x interface the neighbour reads
+    for (auto& v : s.vars)
+        if (const Dim* dx = v.domain_dim(0)) wx = std::max({wx, dx->spec.halo_l, dx->spec.halo_r});
+    const bool fused_ok = !opt_off("fused_halo") && !(points && points_source_near_x_interface(s, t, wx));
 
     // ---- fused path -----------------------------------------------------------------------------------------
     s.fused_x = Solution::FusedX();
     unsigned long long *fx_flag_lo = nullptr, *fx_flag_hi = nullptr;      // the neighbours' flag words (copy-engine path)
     bool only_x = !h->nbrs.empty();
     for (auto& nb : h->nbrs) only_x = only_x && nb.dir[1] == 0 && nb.dir[2] == 0;
-    if (sp.outputs.size() == 1 && !opt_off("fused_halo")) {
+    if (sp.outputs.size() == 1 && fused_ok) {
         const int vi = sp.outputs[0];
         const Var& v = s.vars[vi];
         const int slot = v.slot_of(t + sp.out_step_off);
@@ -556,6 +569,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         const bool signalled = s.fused_x.used && s.fused_x.signalled;
         const bool dma = signalled && fx.dma;
         s.fused_x = Solution::FusedX();
+        if (int e = apply_points(PTS_ALL, whole); e < 0) return e;
         if (dma) {
             const Var& v = s.vars[fx.var];
             const Dim* dx = v.domain_dim(0);
@@ -609,6 +623,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         if (rc < 0) return rc;
         s.stats.kernel_launches += rc;
         mark_outputs_dirty();
+        if (int e = apply_points(PTS_ALL, whole); e < 0) return e;
         return halo_exchange_impl(s, st, -1, false);
     }
     Box cur = whole;
@@ -624,10 +639,12 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         cur.b[d] = interior.b[d]; cur.e[d] = interior.e[d];
     }
     mark_outputs_dirty();
+    if (int e = apply_points(PTS_EXTERIOR, interior); e < 0) return e;
     if (int rc = halo_exchange_impl(s, st, -1, false, true)) return rc;      // pushes on the side stream, behind the exterior
     int rc = s.engine->launch(s, stage, t, interior, st);
     if (rc < 0) return rc;
     s.stats.kernel_launches += rc;
+    if (int e = apply_points(PTS_INTERIOR, interior); e < 0) return e;
     return 0;
 }
 

@@ -1,0 +1,399 @@
+// Point sources and receivers on the device (yb_points.h): one small launch per computed step adds the source wavelet at a
+// few points and records the field at the receiver points, so that a whole shot runs in one run_solution() call instead of
+// the reference API loop run_solution(t, t) / add_to_element / get_element, which pays host round trips on every step.
+#include <stdio.h>
+#include <string.h>
+
+#include <map>
+
+#include "yb_points.h"
+
+namespace yb {
+
+namespace {
+
+struct PointArgs {
+    void* src_slot;                 // step slot of the source var (null: no source row this step)
+    const long long* grp_off;
+    const long long* grp_loc;
+    const int* grp_first;
+    const int* src_col;
+    const double* amp_row;          // amp[u - t0]
+    int ngrp;
+    const void* rcv_slot;           // step slot of the receiver var (null: no receiver row this step)
+    const long long* rcv_off;
+    const long long* rcv_loc;
+    const int* rcv_col;
+    void* trace_row;                // trace[u - t0r]
+    int nrcv;
+    int sel;                        // PTS_*
+    long long ib[3], ie[3];         // interior box (rank-local) for PTS_EXTERIOR / PTS_INTERIOR
+};
+
+__device__ __forceinline__ bool selected(const PointArgs& a, const long long* loc) {
+    if (a.sel == PTS_ALL) return true;
+    const bool in = loc[0] >= a.ib[0] && loc[0] < a.ie[0] && loc[1] >= a.ib[1] && loc[1] < a.ie[1] && loc[2] >= a.ib[2] && loc[2] < a.ie[2];
+    return a.sel == PTS_INTERIOR ? in : !in;
+}
+
+// the rounding of yk_var::add_to_element: the sum is formed in the element type
+__device__ __forceinline__ float add_amp(float v, double a) { return __fadd_rn(v, __double2float_rn(a)); }
+__device__ __forceinline__ double add_amp(double v, double a) { return __dadd_rn(v, a); }
+
+// ONE CTA: a thread applies every source of one point in list order (the host grouped duplicates, so no two threads touch one
+// element and no atomics reorder the adds), the CTA barrier makes the sums visible, then the receivers are read.  Offsets are
+// 64-bit: a slot may hold more than 2^31 elements.
+template <typename T>
+__global__ void __launch_bounds__(256) points_kernel(PointArgs a) {
+    if (a.src_slot) {
+        T* base = static_cast<T*>(a.src_slot);
+        for (int g = threadIdx.x; g < a.ngrp; g += blockDim.x) {
+            if (!selected(a, a.grp_loc + 3 * g)) continue;
+            T v = base[a.grp_off[g]];
+            for (int k = a.grp_first[g]; k < a.grp_first[g + 1]; k++) v = add_amp(v, a.amp_row[a.src_col[k]]);
+            base[a.grp_off[g]] = v;
+        }
+    }
+    __syncthreads();
+    if (a.rcv_slot) {
+        const T* base = static_cast<const T*>(a.rcv_slot);
+        T* out = static_cast<T*>(a.trace_row);
+        for (int j = threadIdx.x; j < a.nrcv; j += blockDim.x)
+            if (selected(a, a.rcv_loc + 3 * j)) out[a.rcv_col[j]] = base[a.rcv_off[j]];
+    }
+}
+
+const char* set_name(bool src) { return src ? "sources" : "receivers"; }
+
+// The var of a point set: step dim, every domain dim, no misc dim, written by a stage.
+int resolve_var(const Solution& s, bool src, const char* name, int& vi, int& step_off) {
+    if (!name) return set_error(YB_EINVAL, "%s: null var name", set_name(src));
+    vi = -1;
+    for (size_t i = 0; i < s.vars.size(); i++)
+        if (s.vars[i].spec.name == name) vi = int(i);
+    if (vi < 0) return set_error(YB_EINVAL, "%s: var '%s' not found in solution '%s'", set_name(src), name, s.spec.name.c_str());
+    const Var& v = s.vars[vi];
+    if (!v.has_step()) return set_error(YB_EINVAL, "%s: var '%s' has no step dim '%s'", set_name(src), name, s.spec.step_dim.c_str());
+    for (auto& d : v.dims)
+        if (d.spec.kind == DIM_MISC)
+            return set_error(YB_EUNSUPPORTED, "%s: var '%s' has misc dim '%s': vars with misc dims are not supported", set_name(src), name, d.spec.name.c_str());
+    for (int k = 0; k < s.ndd; k++)
+        if (!v.domain_dim(k))
+            return set_error(YB_EINVAL, "%s: var '%s' lacks domain dim '%s'", set_name(src), name, s.spec.domain_dims[k].c_str());
+    bool written = false;
+    for (auto& sp : s.spec.stages)
+        for (int o : sp.outputs)
+            if (o == vi) { written = true; step_off = sp.out_step_off; }
+    if (!written) return set_error(YB_EINVAL, "%s: var '%s' is not written by any stage of '%s'", set_name(src), name, s.spec.name.c_str());
+    return 0;
+}
+
+template <typename V>
+int upload(PointsState& p, V*& dst, const std::vector<V>& src) {
+    dst = nullptr;
+    if (src.empty()) return 0;
+    void* d = nullptr;
+    YB_CUDA(cudaMalloc(&d, src.size() * sizeof(V)));
+    p.dev.push_back(d);
+    YB_CUDA(cudaMemcpy(d, src.data(), src.size() * sizeof(V), cudaMemcpyHostToDevice));
+    dst = static_cast<V*>(d);
+    return 0;
+}
+
+void release_device(PointsState& p) {
+    for (void* d : p.dev) cudaFree(d);
+    p.dev.clear();
+    if (p.d_trace) cudaFree(p.d_trace);
+    p.d_trace = nullptr;
+    p.d_grp_off = p.d_grp_loc = p.d_rcv_off = p.d_rcv_loc = nullptr;
+    p.d_grp_first = p.d_src_col = p.d_rcv_col = nullptr;
+    p.d_amp = nullptr;
+}
+
+}  // namespace
+
+void points_free(PointsState* p) {
+    if (!p) return;
+    release_device(*p);
+    delete p;
+}
+
+void points_preload() {
+    preload_kernel((const void*)points_kernel<float>);
+    preload_kernel((const void*)points_kernel<double>);
+}
+
+bool points_active(const Solution& s) { return s.points && (s.points->src.set || s.points->rcv.set); }
+
+static bool geometry_known(const Solution& s) { return s.prepared || s.geometry_planned; }
+
+int points_check_mode(const Solution& s) {
+    if (!points_active(s) || !geometry_known(s) || !s.multi_rank()) return 0;
+    // fused-pair rank grids keep the temporal tile's spare slots (Engine::plan_storage); after prepare the engine says so itself
+    bool pairs = s.prepared && s.engine->fused_steps(s) > 1;
+    for (auto& v : s.vars) pairs = pairs || v.extra_slots > 0;
+    if (pairs)
+        return set_error(YB_EUNSUPPORTED, "point sources and receivers are not supported on a rank grid in fused-pair mode (block_steps=2 with "
+                                          "mega_block_steps=2): its halos are exchanged once per pair of steps, and the state between the two steps "
+                                          "where a source enters is never stored");
+    return 0;
+}
+
+int points_plan(Solution& s) {
+    if (int rc = points_check_mode(s)) return rc;
+    PointsState& p = *s.points;
+    PointPlan plan;
+    auto locate = [&](const PointSet& ps, bool src, int64_t i, long long& off, long long* loc, bool& own) -> int {
+        const Var& v = s.vars[ps.var];
+        off = 0; own = true;
+        loc[0] = loc[1] = loc[2] = 0;
+        for (int k = 0; k < s.ndd; k++) {
+            const int64_t g = ps.idx[size_t(i) * s.ndd + k];
+            if (g < 0 || g >= s.overall_size[k])
+                return set_error(YB_ERANGE, "%s: point %lld has index %lld in dim '%s', outside the overall domain [0,%lld) (halo and pad cells "
+                                            "are refused)", set_name(src), (long long)i, (long long)g, s.spec.domain_dims[k].c_str(),
+                                 (long long)s.overall_size[k]);
+            const int64_t l = g - s.rank_offset[k];
+            if (l < 0 || l >= s.rank_size[k]) own = false;
+            loc[k] = l;
+            const Dim* d = v.domain_dim(k);
+            off += (l + d->pad_l) * d->stride;
+        }
+        return 0;
+    };
+    if (p.src.set) {
+        // on a rank grid the source enters before the exchange of the LAST stage; a var written earlier would already be published
+        if (s.multi_rank()) {
+            bool last = false;
+            for (int o : s.spec.stages.back().outputs) last = last || o == p.src.var;
+            if (!last)
+                return set_error(YB_EUNSUPPORTED, "sources: on a rank grid the source var '%s' must be written by the last stage of '%s'",
+                                 s.vars[p.src.var].spec.name.c_str(), s.spec.name.c_str());
+        }
+        std::map<long long, int> group_of;
+        std::vector<std::vector<int>> cols;
+        for (int64_t i = 0; i < p.src.n; i++) {
+            long long off, loc[3];
+            bool own;
+            if (int rc = locate(p.src, true, i, off, loc, own)) return rc;
+            if (!own) continue;
+            auto it = group_of.find(off);
+            if (it == group_of.end()) {
+                it = group_of.emplace(off, int(cols.size())).first;
+                cols.emplace_back();
+                plan.grp_off.push_back(off);
+                plan.grp_loc.insert(plan.grp_loc.end(), loc, loc + 3);
+            }
+            cols[it->second].push_back(int(i));
+        }
+        plan.grp_first.push_back(0);
+        for (auto& c : cols) {
+            plan.src_col.insert(plan.src_col.end(), c.begin(), c.end());
+            plan.grp_first.push_back(int(plan.src_col.size()));
+        }
+    }
+    if (p.rcv.set) {
+        plan.owned.assign(size_t(p.rcv.n), 0);
+        for (int64_t j = 0; j < p.rcv.n; j++) {
+            long long off, loc[3];
+            bool own;
+            if (int rc = locate(p.rcv, false, j, off, loc, own)) return rc;
+            if (!own) continue;
+            plan.owned[size_t(j)] = 1;
+            plan.rcv_off.push_back(off);
+            plan.rcv_loc.insert(plan.rcv_loc.end(), loc, loc + 3);
+            plan.rcv_col.push_back(int(j));
+        }
+    }
+    p.plan = std::move(plan);
+    return 0;
+}
+
+int points_begin_run(Solution& s) {
+    if (!points_active(s)) return 0;
+    if (int rc = points_check_mode(s)) return rc;
+    PointsState& p = *s.points;
+    if (!p.stale) return 0;
+    if (int rc = points_plan(s)) return rc;
+    release_device(p);
+    const PointPlan& pl = p.plan;
+    if (p.src.set) {
+        if (int rc = upload(p, p.d_grp_off, pl.grp_off)) return rc;
+        if (int rc = upload(p, p.d_grp_loc, pl.grp_loc)) return rc;
+        if (int rc = upload(p, p.d_grp_first, pl.grp_first)) return rc;
+        if (int rc = upload(p, p.d_src_col, pl.src_col)) return rc;
+        if (int rc = upload(p, p.d_amp, p.src.amp)) return rc;
+    }
+    if (p.rcv.set) {
+        if (int rc = upload(p, p.d_rcv_off, pl.rcv_off)) return rc;
+        if (int rc = upload(p, p.d_rcv_loc, pl.rcv_loc)) return rc;
+        if (int rc = upload(p, p.d_rcv_col, pl.rcv_col)) return rc;
+        const size_t bytes = size_t(p.rcv.nrows) * size_t(p.rcv.n) * s.spec.elem_bytes;
+        if (bytes) {
+            YB_CUDA(cudaMalloc(&p.d_trace, bytes));
+            YB_CUDA(cudaMemset(p.d_trace, 0, bytes));
+        }
+    }
+    p.stale = false;
+    return 0;
+}
+
+static bool in_box(const long long* loc, const Box& b) {
+    for (int k = 0; k < 3; k++)
+        if (loc[k] < b.b[k] || loc[k] >= b.e[k]) return false;
+    return true;
+}
+
+int points_launch(Solution& s, int64_t t, int sel, const Box& interior, cudaStream_t st) {
+    if (!points_active(s)) return 0;
+    PointsState& p = *s.points;
+    const PointPlan& pl = p.plan;
+    auto wanted = [&](const long long* loc) { return sel == PTS_ALL || (sel == PTS_INTERIOR) == in_box(loc, interior); };
+    PointArgs a{};
+    a.sel = sel;
+    for (int k = 0; k < 3; k++) { a.ib[k] = interior.b[k]; a.ie[k] = interior.e[k]; }
+    int nsel = 0;
+    if (p.src.set && !pl.grp_off.empty()) {
+        const int64_t u = t + p.src.step_off, row = u - p.src.t0;
+        if (row >= 0 && row < p.src.nrows) {
+            for (size_t g = 0; g < pl.grp_off.size() && !nsel; g++) nsel += wanted(&pl.grp_loc[3 * g]);
+            const Var& v = s.vars[p.src.var];
+            a.src_slot = v.slot_ptr(v.slot_of(u));
+            a.grp_off = p.d_grp_off; a.grp_loc = p.d_grp_loc; a.grp_first = p.d_grp_first; a.src_col = p.d_src_col;
+            a.amp_row = p.d_amp + row * p.src.n;
+            a.ngrp = int(pl.grp_off.size());
+        }
+    }
+    int rsel = 0;
+    if (p.rcv.set && !pl.rcv_off.empty()) {
+        const int64_t u = t + p.rcv.step_off, row = u - p.rcv.t0;
+        if (row >= 0 && row < p.rcv.nrows) {
+            for (size_t j = 0; j < pl.rcv_off.size() && !rsel; j++) rsel += wanted(&pl.rcv_loc[3 * j]);
+            const Var& v = s.vars[p.rcv.var];
+            a.rcv_slot = v.slot_ptr(v.slot_of(u));
+            a.rcv_off = p.d_rcv_off; a.rcv_loc = p.d_rcv_loc; a.rcv_col = p.d_rcv_col;
+            a.trace_row = static_cast<char*>(p.d_trace) + size_t(row) * size_t(p.rcv.n) * s.spec.elem_bytes;
+            a.nrcv = int(pl.rcv_off.size());
+        }
+    }
+    if (!nsel && !rsel) return 0;
+    if (s.spec.elem_bytes == 4) points_kernel<float><<<1, 256, 0, st>>>(a);
+    else points_kernel<double><<<1, 256, 0, st>>>(a);
+    YB_CUDA(cudaGetLastError());
+    p.launches++;
+    return 1;
+}
+
+std::string points_groups_text(const Solution& s) {
+    std::string out;
+    if (!points_active(s)) return out;
+    const PointPlan& pl = s.points->plan;
+    for (size_t g = 0; g + 1 < pl.grp_first.size(); g++) {
+        if (g) out += ';';
+        for (int k = pl.grp_first[g]; k < pl.grp_first[g + 1]; k++) out += (k > pl.grp_first[g] ? "," : "") + std::to_string(pl.src_col[k]);
+    }
+    return out;
+}
+
+bool points_source_near_x_interface(const Solution& s, int64_t t, int64_t w) {
+    if (!points_active(s) || !s.points->src.set) return false;
+    const PointsState& p = *s.points;
+    const int64_t row = t + p.src.step_off - p.src.t0;
+    if (row < 0 || row >= p.src.nrows) return false;
+    const bool lo = s.rank_index[0] > 0, hi = s.rank_index[0] < s.num_ranks[0] - 1;
+    for (size_t g = 0; g < p.plan.grp_off.size(); g++) {
+        const long long x = p.plan.grp_loc[3 * g];
+        if ((lo && x < w) || (hi && x >= s.rank_size[0] - w)) return true;
+    }
+    return false;
+}
+
+}  // namespace yb
+
+using namespace yb;
+
+extern "C" {
+
+#define SOL(s) reinterpret_cast<Solution*>(s)
+
+static int set_points(Solution* s, bool src, const char* var, int64_t n, const int64_t* idx, int64_t t0, int64_t nrows, const double* amp) {
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    if (n < 1) return set_error(YB_EINVAL, "%s: at least one point is needed (clear_points() removes a set)", set_name(src));
+    if (!idx) return set_error(YB_EINVAL, "%s: null index array", set_name(src));
+    if (nrows < 0) return set_error(YB_EINVAL, "%s: negative row count %lld", set_name(src), (long long)nrows);
+    if (src && nrows > 0 && !amp) return set_error(YB_EINVAL, "sources: null amplitude table for %lld rows", (long long)nrows);
+    if (n > int64_t(1) << 30) return set_error(YB_EINVAL, "%s: too many points", set_name(src));
+    PointSet ps;
+    if (int rc = resolve_var(*s, src, var, ps.var, ps.step_off)) return rc;
+    ps.set = true;
+    ps.n = n; ps.t0 = t0; ps.nrows = nrows;
+    ps.idx.assign(idx, idx + size_t(n) * s->ndd);
+    if (src) ps.amp.assign(amp, amp + size_t(nrows) * size_t(n));
+    const bool had = s->points != nullptr;
+    if (!had) s->points = new PointsState();
+    PointSet keep = src ? s->points->src : s->points->rcv;
+    (src ? s->points->src : s->points->rcv) = std::move(ps);
+    s->points->stale = true;
+    // with the rank geometry known the set is checked now (range, ownership, mode); a prepared solution uploads it now too, so
+    // that run_solution() enqueues nothing but launches
+    if (geometry_known(*s)) {
+        if (int rc = points_plan(*s)) {
+            (src ? s->points->src : s->points->rcv) = std::move(keep);
+            return rc;
+        }
+    }
+    if (s->prepared) {
+        YB_CUDA(cudaSetDevice(s->device));
+        YB_CUDA(cudaStreamSynchronize(s->stream()));     // the tables being replaced may still be in use
+        return points_begin_run(*s);
+    }
+    return 0;
+}
+
+int yb_solution_set_sources(yb_solution* s, const char* var, int64_t n, const int64_t* idx, int64_t t0, int64_t nrows, const double* amp) {
+    return set_points(SOL(s), true, var, n, idx, t0, nrows, amp);
+}
+
+int yb_solution_set_receivers(yb_solution* s, const char* var, int64_t m, const int64_t* idx, int64_t t0r, int64_t nrows_r) {
+    return set_points(SOL(s), false, var, m, idx, t0r, nrows_r, nullptr);
+}
+
+int yb_solution_get_traces(yb_solution* s_, void* out, uint8_t* owned) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    if (!points_active(*s) || !s->points->rcv.set) return set_error(YB_ESTATE, "get_traces: no receivers are set");
+    PointsState& p = *s->points;
+    if (p.stale) {
+        if (!geometry_known(*s)) return set_error(YB_ESTATE, "get_traces: the rank geometry is not known yet (plan_geometry / prepare_solution)");
+        if (int rc = points_plan(*s)) return rc;
+    }
+    if (owned) memcpy(owned, p.plan.owned.data(), p.plan.owned.size());
+    if (!out) return 0;
+    const size_t bytes = size_t(p.rcv.nrows) * size_t(p.rcv.n) * s->spec.elem_bytes;
+    if (p.stale || !p.d_trace) {         // nothing recorded since the last change
+        memset(out, 0, bytes);
+        return 0;
+    }
+    YB_CUDA(cudaSetDevice(s->device));
+    YB_CUDA(cudaMemcpyAsync(out, p.d_trace, bytes, cudaMemcpyDeviceToHost, s->stream()));
+    YB_CUDA(cudaStreamSynchronize(s->stream()));
+    return 0;
+}
+
+int yb_solution_clear_points(yb_solution* s_) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    if (!s->points) return 0;
+    if (s->prepared) {
+        YB_CUDA(cudaSetDevice(s->device));
+        YB_CUDA(cudaStreamSynchronize(s->stream()));
+    }
+    const int64_t launches = s->points->launches;
+    points_free(s->points);
+    s->points = new PointsState();
+    s->points->launches = launches;
+    s->points->stale = false;
+    return 0;
+}
+
+}  // extern "C"

@@ -5,6 +5,7 @@
 // factory hands out play the role of StencilContext / YkVarImpl
 // (/root/reference/src/kernel/lib/{factory,soln_apis,yk_var_apis}.cpp).  Host bookkeeping only.
 #include "../include/yask_kernel_api.hpp"
+#include "../include/yask_b200_points.hpp"
 
 #include <cstdlib>
 #include <cstring>
@@ -465,6 +466,7 @@ struct B200Solution : yk_solution {
     std::vector<hook_fn_2idx_t> before_run, after_run;
     bool step_wrap = false;
     int device = -1;
+    idx_t point_rcv = 0, point_rows = 0;   // shape of the receiver set (yk_set_receivers)
 
     // The reference fixes a solution's radius and element size when it builds the kernel library (`make stencil=iso3dfd
     // radius=2 real_bytes=8`, /root/reference/src/kernel/Makefile); here the library name carries them the same way:
@@ -788,6 +790,74 @@ yk_solution_ptr yk_factory::new_solution(yk_env_ptr env, const yk_solution_ptr s
         s->set_rank_index_vec(source->get_rank_index_vec());
     }
     return s;
+}
+
+// ---- point sources and receivers (yask_b200_points.hpp) ----------------------------------------------------------
+namespace {
+B200Solution& b200(const yk_solution_ptr& soln) {
+    auto* s = dynamic_cast<B200Solution*>(soln.get());
+    if (!s) fail("point sources and receivers: not a solution of this engine");
+    return *s;
+}
+std::vector<int64_t> flat_points(B200Solution& s, const std::vector<idx_t_vec>& idx, const char* what) {
+    const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
+    std::vector<int64_t> out;
+    for (size_t i = 0; i < idx.size(); i++) {
+        if (idx[i].size() != nd)
+            fail(std::string(what) + ": point " + std::to_string(i) + " has " + std::to_string(idx[i].size()) + " indices but the solution has " +
+                 std::to_string(nd) + " domain dims");
+        out.insert(out.end(), idx[i].begin(), idx[i].end());
+    }
+    return out;
+}
+}  // namespace
+
+void yk_set_sources(yk_solution_ptr soln, const std::string& var, const std::vector<idx_t_vec>& idx, idx_t t0,
+                    const std::vector<std::vector<double>>& amp) {
+    B200Solution& s = b200(soln);
+    const std::vector<int64_t> pts = flat_points(s, idx, "sources");
+    std::vector<double> flat;
+    for (size_t r = 0; r < amp.size(); r++) {
+        if (amp[r].size() != idx.size())
+            fail("sources: amplitude row " + std::to_string(r) + " has " + std::to_string(amp[r].size()) + " values for " + std::to_string(idx.size()) +
+                 " source point(s)");
+        flat.insert(flat.end(), amp[r].begin(), amp[r].end());
+    }
+    chk(yb_solution_set_sources(s.h->s, var.c_str(), int64_t(idx.size()), pts.data(), t0, int64_t(amp.size()), flat.data()));
+}
+
+void yk_set_receivers(yk_solution_ptr soln, const std::string& var, const std::vector<idx_t_vec>& idx, idx_t t0, idx_t nrows) {
+    B200Solution& s = b200(soln);
+    const std::vector<int64_t> pts = flat_points(s, idx, "receivers");
+    chk(yb_solution_set_receivers(s.h->s, var.c_str(), int64_t(idx.size()), pts.data(), t0, nrows));
+    s.point_rcv = idx_t(idx.size());
+    s.point_rows = nrows;
+}
+
+void yk_get_traces(yk_solution_ptr soln, std::vector<std::vector<double>>& traces, std::vector<bool>& owned) {
+    B200Solution& s = b200(soln);
+    const size_t m = size_t(s.point_rcv), rows = size_t(s.point_rows);
+    const int eb = yb_solution_elem_bytes(s.h->s);
+    std::vector<char> raw(rows * m * eb);
+    std::vector<uint8_t> own(m);
+    chk(yb_solution_get_traces(s.h->s, yb_solution_is_prepared(s.h->s) ? raw.data() : nullptr, own.data()));
+    traces.assign(rows, std::vector<double>(m, 0.0));
+    for (size_t r = 0; r < rows; r++)
+        for (size_t j = 0; j < m; j++)
+            traces[r][j] = eb == 4 ? double(reinterpret_cast<const float*>(raw.data())[r * m + j]) : reinterpret_cast<const double*>(raw.data())[r * m + j];
+    owned.assign(own.begin(), own.end());
+}
+
+void yk_clear_points(yk_solution_ptr soln) {
+    B200Solution& s = b200(soln);
+    chk(yb_solution_clear_points(s.h->s));
+    s.point_rcv = s.point_rows = 0;
+}
+
+idx_t yk_get_point_launches(yk_solution_ptr soln) {
+    char v[64];
+    chk(yb_get_option(b200(soln).h->s, "point_launches", v, sizeof v));
+    return idx_t(atoll(v));
 }
 
 }  // namespace yask

@@ -18,6 +18,7 @@
 #include <cstdint>
 
 #include "../include/yask_kernel_api.hpp"
+#include "../include/yask_b200_points.hpp"
 
 namespace py = pybind11;
 using namespace yask;
@@ -280,4 +281,16 @@ PYBIND11_MODULE(yask_kernel, m) {
         .def("set_step_wrap", &yk_solution::set_step_wrap)
         .def("get_step_wrap", &yk_solution::get_step_wrap)
         .def("set_debug_output", &yk_solution::set_debug_output);
+
+    // ---- point sources and receivers on the device (yask_b200_points.hpp; not in the reference API) ----
+    m.def("yk_set_sources", &yk_set_sources, py::arg("soln"), py::arg("var"), py::arg("idx"), py::arg("t0"), py::arg("amp"));
+    m.def("yk_set_receivers", &yk_set_receivers, py::arg("soln"), py::arg("var"), py::arg("idx"), py::arg("t0"), py::arg("nrows"));
+    m.def("yk_get_traces", [](yk_solution_ptr s) {
+        std::vector<std::vector<double>> traces;
+        std::vector<bool> owned;
+        yk_get_traces(s, traces, owned);
+        return py::make_tuple(traces, owned);
+    }, py::arg("soln"), "(traces[row][receiver] as floats, owned[receiver])");
+    m.def("yk_clear_points", &yk_clear_points, py::arg("soln"));
+    m.def("yk_get_point_launches", &yk_get_point_launches, py::arg("soln"));
 }
