@@ -128,6 +128,7 @@ struct AvpEngine : Engine {
     // option must be set before prepare_solution(); later changes only switch the launch path.  One rank only.
     int block_steps = 1;
     int64_t tt_launches = 0;       // read-only option tt_launches: fused launches since prepare
+    int64_t sweep_launches = 0;    // read-only option gen_sweep_launches (the generated engines' name): one-step sweeps since prepare
     bool tt_ok = false;            // spare slots allocated and tensor maps built
     CUtensorMap tt_maps[4];        // A(t) in each storage slot, the tile's boxes
 
@@ -155,6 +156,7 @@ struct AvpEngine : Engine {
         else if (k == "grid") v = std::to_string(grid_override);
         else if (k == "block_steps") v = std::to_string(block_steps);
         else if (k == "tt_launches") v = std::to_string(tt_launches);
+        else if (k == "gen_sweep_launches") v = std::to_string(sweep_launches);
         else return false;
         return true;
     }
@@ -185,7 +187,7 @@ struct AvpEngine : Engine {
         if (s.spec.elem_bytes != 4 && s.spec.elem_bytes != 8) return set_error(YB_EUNSUPPORTED, "%s: elements must be 4 or 8 bytes", s.spec.name.c_str());
         f64 = s.spec.elem_bytes == 8;
         maps_ok = attr_set = tt_ok = false;
-        tt_launches = 0;
+        tt_launches = sweep_launches = 0;
         cudaDeviceProp prop;
         YB_CUDA(cudaGetDeviceProperties(&prop, s.device));
         num_sms = prop.multiProcessorCount;
@@ -262,6 +264,7 @@ struct AvpEngine : Engine {
             chunk_partition(box.b[0], nxb, P.nchunks, false, false, P.cx0, P.clen, nullptr);
             const int grid = int(std::min<int64_t>(ntile * P.nchunks, g));
             c.fn<<<grid, c.threads, c.smem, st>>>(maps[a.slot_of(t)], P);
+            sweep_launches++;
         } else {
             dim3 grd(unsigned((box.e[2] - box.b[2] + 127) / 128), unsigned(box.e[1] - box.b[1]), unsigned(box.e[0] - box.b[0]));
             if (grd.y > 65535 || grd.z > 65535) return set_error(YB_EUNSUPPORTED, "direct kernel: domain too large in x or y");

@@ -84,6 +84,27 @@ static int compute_rank_geometry(Solution& s) {
     return 0;
 }
 
+// Every rank of a split dim must be at least as wide as the widest halo of the solution's vars in that dim, or a halo exchange
+// would have to send planes it does not own (/root/reference/src/kernel/lib/setup.cpp:709-713, 764-772).  The test is on the
+// grid's smallest rank -- the last one, which takes the remainder -- so that every rank refuses the grid, not only the thin one:
+// a rank prepared alongside a refused neighbour would wait for it forever in its first exchange.
+static int check_min_rank_size(const Solution& s) {
+    for (int d = 0; d < s.ndd; d++) {
+        const int64_t nr = s.num_ranks[d];
+        if (nr <= 1) continue;
+        int64_t halo = 0;
+        for (const Var& v : s.vars)
+            if (!v.spec.user_var)
+                if (const Dim* dd = v.domain_dim(d)) halo = std::max({halo, dd->spec.halo_l, dd->spec.halo_r});
+        const int64_t os = s.overall_size[d];
+        const int64_t smallest = std::min(s.rank_size[d], os - (os + nr - 1) / nr * (nr - 1));
+        if (smallest < halo)
+            return set_error(YB_EINVAL, "local-domain size of %lld in '%s' dim is less than minimum size of %lld, which is based on stencil "
+                                        "halos and temporal wave-front sizes", (long long)smallest, s.spec.domain_dims[d].c_str(), (long long)halo);
+    }
+    return 0;
+}
+
 void compute_var_geometry(Solution& s, Var& v) {
     const int align_elems = 128 / v.elem_bytes;  // 128-B rows
     int nd = int(v.dims.size());
@@ -427,6 +448,7 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     if (!s) return set_error(YB_EINVAL, "null solution");
     if (s->prepared) return 0;
     if (int rc = compute_rank_geometry(*s)) return rc;
+    if (int rc = check_min_rank_size(*s)) return rc;
     plan_storage(*s);
     for (auto& v : s->vars) compute_var_geometry(*s, v);
     s->geometry_planned = true;
@@ -442,6 +464,7 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (ndev <= 0) return set_error(YB_ECUDA, "no CUDA device available: the yask_b200 engine has no CPU fallback");
     if (device < 0 || device >= ndev) return set_error(YB_EINVAL, "device %d out of range [0,%d)", device, ndev);
     if (int rc = compute_rank_geometry(*s)) return rc;
+    if (int rc = check_min_rank_size(*s)) return rc;
     s->geometry_planned = true;
     plan_storage(*s);
     // a size the kernels cannot address is refused before any storage is allocated
