@@ -230,6 +230,29 @@ int yb_solution_set_receivers(yb_solution* s, const char* var, int64_t m, const 
 int yb_solution_get_traces(yb_solution* s, void* out, uint8_t* owned);
 int yb_solution_clear_points(yb_solution* s);      /* remove both sets */
 
+/* ---- slice recorders: boxes of a var recorded on the device inside run_solution() ----------------------------------
+ * Replaces the host loop run_solution(t, t); get_elements_in_slice(frame, {u, first...}, {u, last...}) with one call, for receiver
+ * planes, decimated snapshots and field dumps every k steps.  A recorder records the decimated box first[d], first[d] + stride[d],
+ * ... <= last[d] (num_domain_dims GLOBAL domain indices each, inclusive, inside the overall domain: halo and pad cells are refused;
+ * stride may be NULL for 1 in every dim; the phase comes from the global first, never from a rank's origin).  Whenever a run has
+ * computed step u (after all its stages, and after that step's sources and receivers; u = t+1, or t-1 for a reverse solution),
+ * if u - t0 is a multiple of `every` and r = (u - t0) / every is in [0, nrows): frame[r] = var(u, box) in the element type.
+ * The var must have the step dim and every domain dim, no misc dim, and be written by a stage.  Each rank allocates nrows x its
+ * OWNED part of the decimated box on the device: at this call on a prepared solution (which synchronizes its stream), otherwise
+ * at prepare -- never in run_solution(); an allocation that fails is refused, naming the bytes.  Rows not recorded yet are 0.
+ * Recorders persist across runs until cleared; *id (0, 1, ...) names this one.  While any is set every run takes one step per
+ * launch (block_steps pairs resume once they are cleared); a rank grid whose halos are exchanged once per pair of steps
+ * (block_steps=2 + mega_block_steps=2) refuses them.  Read-only option slice_launches: recording launches since prepare (one per
+ * step in which some recorder of this rank has a row due, whatever the number of recorders). */
+int yb_solution_add_slice(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                          int64_t t0, int64_t every, int64_t nrows, int64_t* id);
+/* Copy the frames of recorder `id` into `out`: nrows x the full decimated box (extents (last - first) / stride + 1, domain dims in
+ * order, the last fastest) of the solution's type; the points this rank does not own stay 0.  owned[] gets 1 per point of the
+ * decimated box this rank records (0 elsewhere).  `out` may be NULL: then only the mask, which needs no device once the rank
+ * geometry is known (plan_geometry). */
+int yb_solution_get_slice_frames(yb_solution* s, int64_t id, void* out, uint8_t* owned);
+int yb_solution_clear_slices(yb_solution* s);      /* remove every recorder and free its frames; ids restart at 0 */
+
 /* ---- multi-GPU halo exchange, one process per GPU (replaces exchange_halos, halo.cpp:80-491) --- */
 /* Each rank exports an opaque blob (CUDA IPC handles of its var storage + sync flags), the
  * launcher all-gathers the blobs (torch.distributed / MPI / files) and imports every

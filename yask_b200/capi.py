@@ -61,7 +61,8 @@ ABI_SYMBOLS = [
     "yb_var_set_slice", "yb_var_get_slice", "yb_var_set_slice_device", "yb_var_get_slice_device", "yb_var_set_all_same",
     "yb_var_set_slice_same", "yb_var_reduce_slice", "yb_solution_auto_tune", "yb_solution_reset_auto_tuner", "yb_solution_is_auto_tuner_enabled", "yb_solution_auto_tuner_report", "yb_var_fill_hash", "yb_var_fill_hash_shifted", "yb_var_checksum", "yb_var_device_ptr", "yb_copy_to_host", "yb_solution_run", "yb_solution_sync",
     "yb_get_stats", "yb_clear_stats", "yb_solution_set_sources", "yb_solution_set_receivers", "yb_solution_get_traces",
-    "yb_solution_clear_points", "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
+    "yb_solution_clear_points", "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
+    "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
 ]
@@ -130,6 +131,9 @@ def lib() -> C.CDLL:
         L.yb_solution_set_receivers.argtypes = [p, C.c_char_p, i64, C.POINTER(i64), i64, i64]
         L.yb_solution_get_traces.argtypes = [p, p, C.POINTER(C.c_uint8)]
         L.yb_solution_clear_points.argtypes = [p]
+        L.yb_solution_add_slice.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, C.POINTER(i64)]
+        L.yb_solution_get_slice_frames.argtypes = [p, i64, p, C.POINTER(C.c_uint8)]
+        L.yb_solution_clear_slices.argtypes = [p]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
         L.yb_halo_export.argtypes = [p, p, C.c_size_t]
         L.yb_halo_import.argtypes = [p, i64, p, C.c_size_t]
@@ -442,6 +446,41 @@ class Solution:
     def clear_points(self):
         _chk(lib().yb_solution_clear_points(self._h))
         self._nrcv = self._nrows_r = 0
+
+    # slice recorders (yb_solution_add_slice / get_slice_frames / clear_slices)
+    def add_slice(self, var: str, first, last, t0: int, nrows: int, stride=None, every: int = 1) -> int:
+        """Record the box first[d], first[d] + stride[d], ... <= last[d] (global domain indices) of var(u) into frame row
+        (u - t0) // every after every step u a run computes with u - t0 a multiple of `every` and the row below nrows.
+        Returns the recorder's id."""
+        nd = len(self.get_domain_dim_names())
+        f, l = np.atleast_1d(np.asarray(first, np.int64)), np.atleast_1d(np.asarray(last, np.int64))
+        st = np.ones(nd, np.int64) if stride is None else np.atleast_1d(np.asarray(stride, np.int64))
+        for what, a in (("first", f), ("last", l), ("stride", st)):
+            if a.shape != (nd,):
+                raise YaskError(-1, f"slice: {what} needs {nd} domain index(es) ({', '.join(self.get_domain_dim_names())}), "
+                                    f"got {a.tolist()}")
+        rid = C.c_int64(-1)
+        _chk(lib().yb_solution_add_slice(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                         int(t0), int(every), int(nrows), C.byref(rid)))
+        if not hasattr(self, "_slices"):
+            self._slices = {}
+        self._slices[rid.value] = (tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1), int(nrows))
+        return rid.value
+
+    def get_slice_frames(self, rid: int):
+        """(frames, owned): frames (nrows, *box_shape) in the element dtype, owned (box_shape) True for the points this rank
+        records; the others stay 0."""
+        shape, nrows = getattr(self, "_slices", {}).get(rid, ((0,), 0))
+        dt = np.float32 if self.get_element_bytes() == 4 else np.float64
+        out = np.zeros((nrows,) + shape, dtype=dt)
+        owned = np.zeros(shape, dtype=np.uint8)
+        _chk(lib().yb_solution_get_slice_frames(self._h, int(rid), out.ctypes.data if self.is_prepared() else None,
+                                                owned.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return out, owned.astype(bool)
+
+    def clear_slices(self):
+        _chk(lib().yb_solution_clear_slices(self._h))
+        self._slices = {}
 
     def is_prepared(self) -> bool:
         return bool(lib().yb_solution_is_prepared(self._h))

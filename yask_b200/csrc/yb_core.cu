@@ -12,6 +12,7 @@
 #include "yb_core.h"
 #include "yb_halo.h"
 #include "yb_points.h"
+#include "yb_slices.h"
 
 namespace yb {
 
@@ -41,6 +42,7 @@ Solution::~Solution() {
         if (comm_stream) cudaStreamDestroy(comm_stream);
     }
     points_free(points);     // device tables are released on `device`, selected above
+    slices_free(slices);
 }
 
 static int check_dim(const Solution* s, int dim) {
@@ -403,7 +405,7 @@ int yb_set_option(yb_solution* s_, const char* key, const char* value) {
     } else if (k == "auto_tune") {
         s->tuner = Solution::InRunTuner();
         s->tuner.enabled = atoi(value) != 0;
-    } else if (k == "point_launches" || k == "point_groups") {
+    } else if (k == "point_launches" || k == "point_groups" || k == "slice_launches") {
         return set_error(YB_EINVAL, "option '%s' is read-only", key);
     } else if (k == "overlap_comms" || k == "min_exterior" || k == "fused_halo" || k == "dma_halo") {
         // consumed by the halo engine at run time
@@ -420,6 +422,7 @@ int yb_get_option(const yb_solution* s_, const char* key, char* value, size_t n)
     if (std::string(key) == "fp_mode") v = std::to_string(s->fp_mode);
     else if (std::string(key) == "point_launches") v = std::to_string(s->points ? s->points->launches : 0);   // read-only
     else if (std::string(key) == "point_groups") v = points_groups_text(*s);                                    // read-only
+    else if (std::string(key) == "slice_launches") v = std::to_string(s->slices ? s->slices->launches : 0);   // read-only
     else if (!s->engine->get_option(*s, key, v)) {
         auto it = s->options.find(key);
         if (it == s->options.end()) return set_error(YB_EINVAL, "unknown option '%s'", key);
@@ -453,7 +456,9 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     for (auto& v : s->vars) compute_var_geometry(*s, v);
     s->geometry_planned = true;
     if (int rc = s->engine->check_geometry(*s)) return rc;
-    return points_active(*s) ? points_plan(*s) : 0;      // point sets given before the geometry are checked now
+    if (points_active(*s))
+        if (int rc = points_plan(*s)) return rc;          // point sets given before the geometry are checked now
+    return slices_plan(*s);                               // and so are slice recorders
 }
 
 int yb_solution_prepare(yb_solution* s_, int device) {
@@ -471,6 +476,7 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     for (auto& v : s->vars)
         if (!v.dev) compute_var_geometry(*s, v);
     if (int rc = s->engine->check_geometry(*s)) return rc;
+    if (int rc = slices_plan(*s)) return rc;
     YB_CUDA(cudaSetDevice(device));
     s->device = device;
     if (!s->own_stream) YB_CUDA(cudaStreamCreateWithFlags(&s->own_stream, cudaStreamNonBlocking));
@@ -492,9 +498,12 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     }
     if (int rc = s->engine->prepare(*s)) return rc;
     points_preload();
+    slices_preload();
     if (s->multi_rank()) {
         if (int rc = halo_prepare(*s)) return rc;
     }
+    if (int rc = slices_prepare(*s)) return rc;       // frames of the recorders added before prepare
+    if (s->slices) s->slices->launches = 0;
     YB_CUDA(cudaStreamSynchronize(s->stream()));
     s->prepared = true;
     memset(&s->stats, 0, sizeof s->stats);
@@ -833,6 +842,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     cudaStream_t st = s->stream();
     // point tables are normally uploaded when they are set (or at prepare); before anything of this run is enqueued otherwise
     if (int rc = points_begin_run(*s)) return rc;
+    if (int rc = slices_begin_run(*s)) return rc;
     // Timing events: pairs of finished runs are folded into the stats and recycled here, so that calling
     // run_solution(t) once per step (the reference's usual pattern) keeps a bounded number of events alive.
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -867,10 +877,10 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward run goes through the engine's fused launch, `fs` steps
     // at a time; what is left over (and every other kind of run) takes the one-step path below.  A rank grid fuses steps only
     // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.  Point sources
-    // enter between two steps, so a solution with points runs one step per launch (points_check_mode refuses them on a rank
-    // grid in the fused mode).
+    // enter between two steps, and slice recorders read a step a pair would never store, so a solution with points or recorders
+    // runs one step per launch (both are refused on a rank grid in the fused mode).
     int64_t t_first = first_step;
-    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s)) ? s->engine->fused_steps(*s) : 1;
+    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s) && !slices_active(*s)) ? s->engine->fused_steps(*s) : 1;
     if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
         const bool ends_run = t_first + fs - 1 == last_step;
@@ -918,6 +928,8 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
         }
         // sources and receivers of the step just computed (a rank grid applies them inside its last stage, halo_run_stage)
         if (rc >= 0 && !s->halo) rc = points_launch(*s, t, PTS_ALL, whole, st);
+        // then the slice recorders, before the next step's first launch can overwrite an in-place var (halo_run_stage on a grid)
+        if (rc >= 0 && !s->halo) rc = slices_launch(*s, t, st);
         s->stats.num_steps_done++;
         if (tv >= 0 && te0 && te1) {
             cudaEventRecord(te1, st);

@@ -173,6 +173,8 @@ struct HaloState;  // yb_halo.cu
 void halo_free(HaloState*);
 struct PointsState;  // yb_points.cu
 void points_free(PointsState*);
+struct SlicesState;  // yb_slices.cu
+void slices_free(SlicesState*);
 
 struct Solution {
     StencilSpec spec;
@@ -217,6 +219,8 @@ struct Solution {
     HaloState* halo = nullptr;   // owned; freed by halo_free()
     // point sources and receivers (yb_points.h)
     PointsState* points = nullptr;   // owned; freed by points_free()
+    // slice recorders (yb_slices.h)
+    SlicesState* slices = nullptr;   // owned; freed by slices_free()
     // Fused halo stores (set by the halo layer before a stage launch, consumed by an engine that can store its
     // boundary planes straight into the x neighbours' halo cells): element (0,0,0)-relative base pointers of the
     // OUTPUT var's step slot in the lower / upper x neighbour, or null.  The engine sets `used` if it honoured them.

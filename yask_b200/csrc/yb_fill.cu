@@ -2,19 +2,12 @@
 // equivalent of YkVarBase::get/set_elements_in_slice, /root/reference/src/kernel/lib/yk_var.hpp:1222-1300),
 // constant fills (set_all_elements_same, yk_var.hpp:1786-1793), the synthetic hash-field
 // generator (yask_b200/synth.py) and an order-independent checksum.
+#include "yb_box.cuh"
 #include "yb_core.h"
 
 namespace yb {
 
 namespace {
-
-struct BoxDev {
-    int nd;
-    long long n[4];
-    long long vs[4];
-    long long off;
-    long long total;
-};
 
 __host__ BoxDev to_dev(const BoxCopy& bc) {
     BoxDev b;
@@ -27,19 +20,6 @@ __host__ BoxDev to_dev(const BoxCopy& bc) {
     }
     b.off = bc.var_off;
     return b;
-}
-
-// dense linear index -> storage element offset; also returns per-dim coordinates
-__device__ __forceinline__ long long box_offset(const BoxDev& b, long long lin, long long* coord) {
-    long long o = b.off;
-#pragma unroll
-    for (int d = 3; d >= 0; d--) {
-        long long c = lin % b.n[d];
-        lin /= b.n[d];
-        coord[d] = c;
-        o += c * b.vs[d];
-    }
-    return o;
 }
 
 template <typename T>

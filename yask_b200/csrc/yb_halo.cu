@@ -25,6 +25,7 @@
 
 #include "yb_halo.h"
 #include "yb_points.h"
+#include "yb_slices.h"
 
 namespace yb {
 
@@ -494,6 +495,9 @@ static bool other_dirty(const HaloState* h, int var, int slot) {
 // than the widest x halo from every x interface (no neighbour reads them).  A rank that owns a source nearer than that runs the
 // stage in the split form instead: the fused launch stores and publishes its boundary planes itself, before a source could enter.
 // Both forms advance the epoch once, so the choice is the rank's own.
+// Slice recorders (yb_slices.h) only read: they record in the last stage, after the launch that computed the rank's last points
+// and that launch's points (fused: the launch; whole: the launch; split: the interior launch), on this stream, so before the next
+// step's first launch overwrites an in-place var.  They never change the form.
 int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     Box whole;
     for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = d < s.ndd ? s.rank_size[d] : 1; }
@@ -508,6 +512,8 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     const bool overlap = !opt_off("overlap_comms");
     const bool points = stage + 1 == int(s.spec.stages.size()) && points_active(s);
     auto apply_points = [&](int sel, const Box& interior) { return points ? points_launch(s, t, sel, interior, st) : 0; };
+    const bool last_stage = stage + 1 == int(s.spec.stages.size());
+    auto record_slices = [&]() { return last_stage ? slices_launch(s, t, st) : 0; };
     int64_t wx = 0;         // widest x halo: the planes of an x interface the neighbour reads
     for (auto& v : s.vars)
         if (const Dim* dx = v.domain_dim(0)) wx = std::max({wx, dx->spec.halo_l, dx->spec.halo_r});
@@ -570,6 +576,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         const bool dma = signalled && fx.dma;
         s.fused_x = Solution::FusedX();
         if (int e = apply_points(PTS_ALL, whole); e < 0) return e;
+        if (int e = record_slices(); e < 0) return e;
         if (dma) {
             const Var& v = s.vars[fx.var];
             const Dim* dx = v.domain_dim(0);
@@ -624,6 +631,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         s.stats.kernel_launches += rc;
         mark_outputs_dirty();
         if (int e = apply_points(PTS_ALL, whole); e < 0) return e;
+        if (int e = record_slices(); e < 0) return e;
         return halo_exchange_impl(s, st, -1, false);
     }
     Box cur = whole;
@@ -645,6 +653,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     if (rc < 0) return rc;
     s.stats.kernel_launches += rc;
     if (int e = apply_points(PTS_INTERIOR, interior); e < 0) return e;
+    if (int e = record_slices(); e < 0) return e;
     return 0;
 }
 

@@ -65,29 +65,6 @@ __global__ void __launch_bounds__(256) points_kernel(PointArgs a) {
 
 const char* set_name(bool src) { return src ? "sources" : "receivers"; }
 
-// The var of a point set: step dim, every domain dim, no misc dim, written by a stage.
-int resolve_var(const Solution& s, bool src, const char* name, int& vi, int& step_off) {
-    if (!name) return set_error(YB_EINVAL, "%s: null var name", set_name(src));
-    vi = -1;
-    for (size_t i = 0; i < s.vars.size(); i++)
-        if (s.vars[i].spec.name == name) vi = int(i);
-    if (vi < 0) return set_error(YB_EINVAL, "%s: var '%s' not found in solution '%s'", set_name(src), name, s.spec.name.c_str());
-    const Var& v = s.vars[vi];
-    if (!v.has_step()) return set_error(YB_EINVAL, "%s: var '%s' has no step dim '%s'", set_name(src), name, s.spec.step_dim.c_str());
-    for (auto& d : v.dims)
-        if (d.spec.kind == DIM_MISC)
-            return set_error(YB_EUNSUPPORTED, "%s: var '%s' has misc dim '%s': vars with misc dims are not supported", set_name(src), name, d.spec.name.c_str());
-    for (int k = 0; k < s.ndd; k++)
-        if (!v.domain_dim(k))
-            return set_error(YB_EINVAL, "%s: var '%s' lacks domain dim '%s'", set_name(src), name, s.spec.domain_dims[k].c_str());
-    bool written = false;
-    for (auto& sp : s.spec.stages)
-        for (int o : sp.outputs)
-            if (o == vi) { written = true; step_off = sp.out_step_off; }
-    if (!written) return set_error(YB_EINVAL, "%s: var '%s' is not written by any stage of '%s'", set_name(src), name, s.spec.name.c_str());
-    return 0;
-}
-
 template <typename V>
 int upload(PointsState& p, V*& dst, const std::vector<V>& src) {
     dst = nullptr;
@@ -112,6 +89,29 @@ void release_device(PointsState& p) {
 
 }  // namespace
 
+// The var of a point set or a slice recorder (`what`): step dim, every domain dim, no misc dim, written by a stage.
+int point_var(const Solution& s, const char* what, const char* name, int& vi, int& step_off) {
+    if (!name) return set_error(YB_EINVAL, "%s: null var name", what);
+    vi = -1;
+    for (size_t i = 0; i < s.vars.size(); i++)
+        if (s.vars[i].spec.name == name) vi = int(i);
+    if (vi < 0) return set_error(YB_EINVAL, "%s: var '%s' not found in solution '%s'", what, name, s.spec.name.c_str());
+    const Var& v = s.vars[vi];
+    if (!v.has_step()) return set_error(YB_EINVAL, "%s: var '%s' has no step dim '%s'", what, name, s.spec.step_dim.c_str());
+    for (auto& d : v.dims)
+        if (d.spec.kind == DIM_MISC)
+            return set_error(YB_EUNSUPPORTED, "%s: var '%s' has misc dim '%s': vars with misc dims are not supported", what, name, d.spec.name.c_str());
+    for (int k = 0; k < s.ndd; k++)
+        if (!v.domain_dim(k))
+            return set_error(YB_EINVAL, "%s: var '%s' lacks domain dim '%s'", what, name, s.spec.domain_dims[k].c_str());
+    bool written = false;
+    for (auto& sp : s.spec.stages)
+        for (int o : sp.outputs)
+            if (o == vi) { written = true; step_off = sp.out_step_off; }
+    if (!written) return set_error(YB_EINVAL, "%s: var '%s' is not written by any stage of '%s'", what, name, s.spec.name.c_str());
+    return 0;
+}
+
 void points_free(PointsState* p) {
     if (!p) return;
     release_device(*p);
@@ -125,14 +125,19 @@ void points_preload() {
 
 bool points_active(const Solution& s) { return s.points && (s.points->src.set || s.points->rcv.set); }
 
-static bool geometry_known(const Solution& s) { return s.prepared || s.geometry_planned; }
+bool geometry_known(const Solution& s) { return s.prepared || s.geometry_planned; }
 
-int points_check_mode(const Solution& s) {
-    if (!points_active(s) || !geometry_known(s) || !s.multi_rank()) return 0;
+bool fused_pair_rank_grid(const Solution& s) {
+    if (!geometry_known(s) || !s.multi_rank()) return false;
     // fused-pair rank grids keep the temporal tile's spare slots (Engine::plan_storage); after prepare the engine says so itself
     bool pairs = s.prepared && s.engine->fused_steps(s) > 1;
     for (auto& v : s.vars) pairs = pairs || v.extra_slots > 0;
-    if (pairs)
+    return pairs;
+}
+
+int points_check_mode(const Solution& s) {
+    if (!points_active(s)) return 0;
+    if (fused_pair_rank_grid(s))
         return set_error(YB_EUNSUPPORTED, "point sources and receivers are not supported on a rank grid in fused-pair mode (block_steps=2 with "
                                           "mega_block_steps=2): its halos are exchanged once per pair of steps, and the state between the two steps "
                                           "where a source enters is never stored");
@@ -324,7 +329,7 @@ static int set_points(Solution* s, bool src, const char* var, int64_t n, const i
     if (src && nrows > 0 && !amp) return set_error(YB_EINVAL, "sources: null amplitude table for %lld rows", (long long)nrows);
     if (n > int64_t(1) << 30) return set_error(YB_EINVAL, "%s: too many points", set_name(src));
     PointSet ps;
-    if (int rc = resolve_var(*s, src, var, ps.var, ps.step_off)) return rc;
+    if (int rc = point_var(*s, set_name(src), var, ps.var, ps.step_off)) return rc;
     ps.set = true;
     ps.n = n; ps.t0 = t0; ps.nrows = nrows;
     ps.idx.assign(idx, idx + size_t(n) * s->ndd);

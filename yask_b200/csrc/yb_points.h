@@ -47,6 +47,12 @@ struct PointsState {
 enum { PTS_ALL = 0, PTS_EXTERIOR = 1, PTS_INTERIOR = 2 };
 
 void points_free(PointsState* p);
+// The var of a point set or a slice recorder (`what` prefixes the messages): step dim, every domain dim, no misc dim, written by
+// a stage; step_off: the step its writing stage computes, relative to t
+int point_var(const Solution& s, const char* what, const char* name, int& vi, int& step_off);
+bool geometry_known(const Solution& s);         // plan_geometry() or prepare_solution() has run
+// a rank grid whose halos are exchanged once per pair of steps (block_steps=2 + mega_block_steps=2), known from plan_geometry()
+bool fused_pair_rank_grid(const Solution& s);
 void points_preload();                       // load the point kernel now (preload_kernel)
 bool points_active(const Solution& s);
 // refuse point sets on a rank grid whose halos are exchanged once per pair of steps (fixed at prepare on every rank)

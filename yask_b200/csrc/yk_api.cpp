@@ -6,6 +6,7 @@
 // (/root/reference/src/kernel/lib/{factory,soln_apis,yk_var_apis}.cpp).  Host bookkeeping only.
 #include "../include/yask_kernel_api.hpp"
 #include "../include/yask_b200_points.hpp"
+#include "../include/yask_b200_slices.hpp"
 
 #include <cstdlib>
 #include <cstring>
@@ -467,6 +468,7 @@ struct B200Solution : yk_solution {
     bool step_wrap = false;
     int device = -1;
     idx_t point_rcv = 0, point_rows = 0;   // shape of the receiver set (yk_set_receivers)
+    std::vector<idx_t_vec> slice_shape;     // frames shape (nrows, box extents...) of each slice recorder (yk_add_slice)
 
     // The reference fixes a solution's radius and element size when it builds the kernel library (`make stencil=iso3dfd
     // radius=2 real_bytes=8`, /root/reference/src/kernel/Makefile); here the library name carries them the same way:
@@ -857,6 +859,60 @@ void yk_clear_points(yk_solution_ptr soln) {
 idx_t yk_get_point_launches(yk_solution_ptr soln) {
     char v[64];
     chk(yb_get_option(b200(soln).h->s, "point_launches", v, sizeof v));
+    return idx_t(atoll(v));
+}
+
+// ---- slice recorders (yask_b200_slices.hpp) ------------------------------------------------------------------------
+namespace {
+B200Solution& b200_slices(const yk_solution_ptr& soln) {
+    auto* s = dynamic_cast<B200Solution*>(soln.get());
+    if (!s) fail("slice recorders: not a solution of this engine");
+    return *s;
+}
+}  // namespace
+
+idx_t yk_add_slice(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0, idx_t nrows,
+                   const idx_t_vec& stride, idx_t every) {
+    B200Solution& s = b200_slices(soln);
+    const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
+    if (first.size() != nd || last.size() != nd || (!stride.empty() && stride.size() != nd))
+        fail("slice: first, last and stride need " + std::to_string(nd) + " domain indices each");
+    const std::vector<int64_t> f(first.begin(), first.end()), l(last.begin(), last.end()), st(stride.begin(), stride.end());
+    int64_t id = -1;
+    chk(yb_solution_add_slice(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, &id));
+    idx_t_vec shape{nrows};
+    for (size_t k = 0; k < nd; k++) shape.push_back((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1);
+    s.slice_shape.resize(size_t(id) + 1);
+    s.slice_shape[size_t(id)] = shape;
+    return idx_t(id);
+}
+
+void yk_get_slice_frames(yk_solution_ptr soln, idx_t id, std::vector<double>& frames, idx_t_vec& shape, std::vector<bool>& owned) {
+    B200Solution& s = b200_slices(soln);
+    if (id < 0 || size_t(id) >= s.slice_shape.size()) fail("get_slice_frames: no slice recorder " + std::to_string(id));
+    shape = s.slice_shape[size_t(id)];
+    size_t box = 1;
+    for (size_t k = 1; k < shape.size(); k++) box *= size_t(shape[k]);
+    const size_t n = size_t(shape[0]) * box;
+    const int eb = yb_solution_elem_bytes(s.h->s);
+    std::vector<char> raw(n * eb);
+    std::vector<uint8_t> own(box);
+    chk(yb_solution_get_slice_frames(s.h->s, id, yb_solution_is_prepared(s.h->s) ? raw.data() : nullptr, own.data()));
+    frames.resize(n);
+    for (size_t i = 0; i < n; i++)
+        frames[i] = eb == 4 ? double(reinterpret_cast<const float*>(raw.data())[i]) : reinterpret_cast<const double*>(raw.data())[i];
+    owned.assign(own.begin(), own.end());
+}
+
+void yk_clear_slices(yk_solution_ptr soln) {
+    B200Solution& s = b200_slices(soln);
+    chk(yb_solution_clear_slices(s.h->s));
+    s.slice_shape.clear();
+}
+
+idx_t yk_get_slice_launches(yk_solution_ptr soln) {
+    char v[64];
+    chk(yb_get_option(b200_slices(soln).h->s, "slice_launches", v, sizeof v));
     return idx_t(atoll(v));
 }
 

@@ -19,6 +19,7 @@
 
 #include "../include/yask_kernel_api.hpp"
 #include "../include/yask_b200_points.hpp"
+#include "../include/yask_b200_slices.hpp"
 
 namespace py = pybind11;
 using namespace yask;
@@ -293,4 +294,17 @@ PYBIND11_MODULE(yask_kernel, m) {
     }, py::arg("soln"), "(traces[row][receiver] as floats, owned[receiver])");
     m.def("yk_clear_points", &yk_clear_points, py::arg("soln"));
     m.def("yk_get_point_launches", &yk_get_point_launches, py::arg("soln"));
+
+    // ---- slice recorders on the device (yask_b200_slices.hpp; not in the reference API) ----
+    m.def("yk_add_slice", &yk_add_slice, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"), py::arg("t0"), py::arg("nrows"),
+          py::arg("stride") = idx_t_vec{}, py::arg("every") = 1);
+    m.def("yk_get_slice_frames", [](yk_solution_ptr s, idx_t id) {
+        std::vector<double> frames;
+        idx_t_vec shape;
+        std::vector<bool> owned;
+        yk_get_slice_frames(s, id, frames, shape, owned);
+        return py::make_tuple(frames, shape, owned);
+    }, py::arg("soln"), py::arg("id"), "(frames as a flat list of floats, shape (nrows, box extents...), owned per box point)");
+    m.def("yk_clear_slices", &yk_clear_slices, py::arg("soln"));
+    m.def("yk_get_slice_launches", &yk_get_slice_launches, py::arg("soln"));
 }

@@ -1,0 +1,32 @@
+// Slice recorders on the device inside run_solution(): an extension of the C++ kernel API of this engine.
+//
+// The reference API has no such calls; its users record a receiver plane or a snapshot from the host, one step at a time:
+//
+//     for (idx_t t = 0; t < nt; t++) {
+//         soln->run_solution(t);
+//         if ((t + 1) % k == 0) p->get_elements_in_slice(frame[(t + 1) / k], {t + 1, x0, y0, z0}, {t + 1, x1, y1, z1});
+//     }
+//
+// With the functions below the same frames come from one soln->run_solution(0, nt - 1) call, bit for bit: after every step u a
+// run computes (and after that step's sources and receivers, yask_b200_points.hpp), if u - t0 is a multiple of `every` and
+// r = (u - t0) / every < nrows, frame r holds var(u) at first[d], first[d] + stride[d], ... <= last[d].  They are free functions,
+// not members: yk_solution keeps the reference's vtable layout.  Semantics, storage and the rank-grid rules:
+// yb_solution_add_slice in include/yask_b200.h.
+#pragma once
+#include "yask_kernel_api.hpp"
+
+namespace yask {
+
+// first, last: global domain indices (x, y, z order of get_domain_dim_names()), inclusive; stride: empty for 1 in every dim.
+// Returns the recorder's id (0, 1, ... until yk_clear_slices).
+idx_t yk_add_slice(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0, idx_t nrows,
+                   const idx_t_vec& stride = {}, idx_t every = 1);
+// frames: nrows x the decimated box, row-major, the last domain dim fastest, widened to double (rows not recorded yet and points
+// this rank does not own are 0); shape: (nrows, box extents...); owned: per box point, this rank records it.
+void yk_get_slice_frames(yk_solution_ptr soln, idx_t id, std::vector<double>& frames, idx_t_vec& shape, std::vector<bool>& owned);
+// Remove every recorder: later runs take their usual launch path again.
+void yk_clear_slices(yk_solution_ptr soln);
+// Recording launches since prepare_solution().
+idx_t yk_get_slice_launches(yk_solution_ptr soln);
+
+}  // namespace yask
