@@ -230,6 +230,36 @@ int yb_solution_set_receivers(yb_solution* s, const char* var, int64_t m, const 
 int yb_solution_get_traces(yb_solution* s, void* out, uint8_t* owned);
 int yb_solution_clear_points(yb_solution* s);      /* remove both sets */
 
+/* Weighted sets: sources and receivers between grid points.  Each of the n sources (m receivers) has k support entries
+ * (idx[i][q], w[i][q]): num_domain_dims GLOBAL domain indices (idx is n x k x num_domain_dims, row-major) and a double weight
+ * (w is n x k).  A weighted set replaces the set of its kind, on-grid or weighted; the source set and the receiver set are each
+ * one kind or the other, independently.  Whenever a run has computed step u (after all its stages):
+ *   1. if 0 <= u - t0 < nrows: for each source i in list order, each entry q in order with w[i][q] != 0:
+ *      a = w[i][q] * amp[u - t0][i] in double (one rounded multiply), added to var(u, idx[i][q]) with add_to_element's rounding
+ *      (fp32: float(float(old) + float(a)); fp64: old + a);
+ *   2. then, if 0 <= u - t0r < nrows_r: for each receiver j, acc = +0.0 (double), then for each entry q in order with
+ *      w[j][q] != 0: acc = acc + w[j][q] * double(var(u, idx[j][q])), every multiply and add rounded on its own (no FMA);
+ *      trace[u - t0r][j] = T(acc), rounded to nearest.
+ * Entries of weight exactly 0 are dropped and need not lie in the domain; every other entry must.  A non-finite weight, k < 1 and
+ * a point whose weights are all 0 are refused.  k = 1, w = 1 gives the bits of yb_solution_set_sources / set_receivers.
+ * On a rank grid each rank adds the source entries of its own domain.  Receiver j is owned (get_traces' mask) by the rank holding
+ * its first nonzero entry; every other entry must be in that rank's domain or in a halo cell its exchange refreshes (within the
+ * var's halo, toward a neighbour the var exchanges with: iso3dfd's p exchanges with face neighbours only, so a receiver reaching a
+ * diagonal neighbour is refused).  A receiver that reads halo cells is recorded after the step's last exchange and needs its var
+ * written by the last stage, and either two step slots or two stages.  Every other rule (var, prepare, upload, pairs, fused-pair
+ * rank grids, get_traces, clear_points) is that of yb_solution_set_sources.  point_launches counts one per kernel launched;
+ * point_groups writes a weighted entry as i/q ("0/3,2/0;1/0"). */
+int yb_solution_set_sources_weighted(yb_solution* s, const char* var, int64_t n, int64_t k, const int64_t* idx, const double* w,
+                                     int64_t t0, int64_t nrows, const double* amp /* nrows x n */);
+int yb_solution_set_receivers_weighted(yb_solution* s, const char* var, int64_t m, int64_t k, const int64_t* idx, const double* w,
+                                       int64_t t0r, int64_t nrows_r);
+/* Trilinear support of n positions of ndd (1-3) doubles each, in global index units (e.g. 511.25): k = 2^ndd entries per point,
+ * idx_out n x k x ndd, w_out n x k.  Per dim d: i_d = floor(p_d), f_d = p_d - i_d.  Entry c (0 .. k-1) takes i_d + bit in dim d,
+ * bit = (c >> (ndd - 1 - d)) & 1 (x varies slowest); its weight is ((1.0 * g_0) * g_1) * g_2 in double, left to right, with
+ * g_d = bit ? f_d : 1.0 - f_d.  An integer position yields one entry of weight 1 and k - 1 of weight 0.  Non-finite positions
+ * (and |p| >= 2^62) are refused.  Needs no solution and no device. */
+int yb_points_trilinear(int ndd, int64_t n, const double* pos, int64_t* idx_out, double* w_out);
+
 /* ---- slice recorders: boxes of a var recorded on the device inside run_solution() ----------------------------------
  * Replaces the host loop run_solution(t, t); get_elements_in_slice(frame, {u, first...}, {u, last...}) with one call, for receiver
  * planes, decimated snapshots and field dumps every k steps.  A recorder records the decimated box first[d], first[d] + stride[d],

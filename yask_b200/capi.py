@@ -61,7 +61,8 @@ ABI_SYMBOLS = [
     "yb_var_set_slice", "yb_var_get_slice", "yb_var_set_slice_device", "yb_var_get_slice_device", "yb_var_set_all_same",
     "yb_var_set_slice_same", "yb_var_reduce_slice", "yb_solution_auto_tune", "yb_solution_reset_auto_tuner", "yb_solution_is_auto_tuner_enabled", "yb_solution_auto_tuner_report", "yb_var_fill_hash", "yb_var_fill_hash_shifted", "yb_var_checksum", "yb_var_device_ptr", "yb_copy_to_host", "yb_solution_run", "yb_solution_sync",
     "yb_get_stats", "yb_clear_stats", "yb_solution_set_sources", "yb_solution_set_receivers", "yb_solution_get_traces",
-    "yb_solution_clear_points", "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
+    "yb_solution_clear_points", "yb_solution_set_sources_weighted", "yb_solution_set_receivers_weighted", "yb_points_trilinear",
+    "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
     "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
@@ -131,6 +132,10 @@ def lib() -> C.CDLL:
         L.yb_solution_set_receivers.argtypes = [p, C.c_char_p, i64, C.POINTER(i64), i64, i64]
         L.yb_solution_get_traces.argtypes = [p, p, C.POINTER(C.c_uint8)]
         L.yb_solution_clear_points.argtypes = [p]
+        L.yb_solution_set_sources_weighted.argtypes = [p, C.c_char_p, i64, i64, C.POINTER(i64), C.POINTER(C.c_double), i64, i64,
+                                                       C.POINTER(C.c_double)]
+        L.yb_solution_set_receivers_weighted.argtypes = [p, C.c_char_p, i64, i64, C.POINTER(i64), C.POINTER(C.c_double), i64, i64]
+        L.yb_points_trilinear.argtypes = [i32, i64, C.POINTER(C.c_double), C.POINTER(i64), C.POINTER(C.c_double)]
         L.yb_solution_add_slice.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, C.POINTER(i64)]
         L.yb_solution_get_slice_frames.argtypes = [p, i64, p, C.POINTER(C.c_uint8)]
         L.yb_solution_clear_slices.argtypes = [p]
@@ -160,6 +165,24 @@ def device_count() -> int:
 
 def version() -> str:
     return lib().yb_version_string().decode()
+
+
+def trilinear(pos):
+    """Trilinear support of real-valued positions in global index units: pos (n, ndd) -> (idx (n, 2^ndd, ndd) int64,
+    w (n, 2^ndd) float64), entry c taking floor(p_d) + bit (ndd - 1 - d) of c in dim d, its weight the product over d, left to
+    right, of f_d or 1 - f_d (yb_points_trilinear).  An integer position gets one entry of weight 1, the rest 0."""
+    a = np.asarray(pos, dtype=np.float64)
+    if a.ndim == 1:
+        a = a.reshape(1, -1)
+    if a.ndim != 2 or not 1 <= a.shape[1] <= 3 or a.shape[0] < 1:
+        raise YaskError(-1, f"trilinear: expected positions of shape (n, ndd) with ndd 1, 2 or 3, got shape {a.shape}")
+    a = np.ascontiguousarray(a)
+    n, nd = a.shape
+    idx = np.zeros((n, 1 << nd, nd), np.int64)
+    w = np.zeros((n, 1 << nd), np.float64)
+    _chk(lib().yb_points_trilinear(nd, n, a.ctypes.data_as(C.POINTER(C.c_double)), idx.ctypes.data_as(C.POINTER(C.c_int64)),
+                                   w.ctypes.data_as(C.POINTER(C.c_double))))
+    return idx, w
 
 
 def _arr(vals: Sequence[int]):
@@ -431,6 +454,40 @@ class Solution:
         pts = self._points(idx, "receivers")
         _chk(lib().yb_solution_set_receivers(self._h, var.encode(), pts.shape[0], pts.ctypes.data_as(C.POINTER(C.c_int64)),
                                              int(t0), int(nrows)))
+        self._nrcv, self._nrows_r = pts.shape[0], int(nrows)
+
+    def _weighted(self, idx, w, what: str):
+        nd = len(self.get_domain_dim_names())
+        a = np.asarray(idx, dtype=np.int64)
+        ww = np.asarray(w, dtype=np.float64)
+        if a.ndim != 3 or a.shape[2] != nd or a.shape[0] < 1 or a.shape[1] < 1:
+            raise YaskError(-1, f"{what}: expected an index table of shape (n, k, {nd}) -- k support entries of {nd} domain "
+                                f"index(es) ({', '.join(self.get_domain_dim_names())}) per point -- got shape {a.shape}")
+        if ww.shape != a.shape[:2]:
+            raise YaskError(-1, f"{what}: weight table of shape {ww.shape} does not match the index table: expected {a.shape[:2]}")
+        return np.ascontiguousarray(a), np.ascontiguousarray(ww)
+
+    def set_sources_weighted(self, var: str, idx, w, t0: int, amp):
+        """Add w[i][q] * amp[u - t0][i] to var(u, idx[i][q]) for every source i in list order and every entry q in order with
+        w[i][q] != 0, after every step u a run computes with 0 <= u - t0 < len(amp).  idx: (N, k, ndd) global domain indices;
+        w: (N, k); amp: (nrows, N)."""
+        pts, ww = self._weighted(idx, w, "weighted sources")
+        a = np.asarray(amp, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != pts.shape[0]:
+            raise YaskError(-1, f"weighted sources: amplitude table of shape {a.shape} does not match {pts.shape[0]} source(s): "
+                                f"expected (nrows, {pts.shape[0]})")
+        a = np.ascontiguousarray(a)
+        _chk(lib().yb_solution_set_sources_weighted(self._h, var.encode(), pts.shape[0], pts.shape[1],
+                                                    pts.ctypes.data_as(C.POINTER(C.c_int64)), ww.ctypes.data_as(C.POINTER(C.c_double)),
+                                                    int(t0), a.shape[0], a.ctypes.data_as(C.POINTER(C.c_double))))
+
+    def set_receivers_weighted(self, var: str, idx, w, t0: int, nrows: int):
+        """Record the sum over q in order of w[j][q] * var(u, idx[j][q]) (in double, each product and sum rounded, then rounded
+        to the element type) into trace row u - t0 after every step u a run computes with 0 <= u - t0 < nrows."""
+        pts, ww = self._weighted(idx, w, "weighted receivers")
+        _chk(lib().yb_solution_set_receivers_weighted(self._h, var.encode(), pts.shape[0], pts.shape[1],
+                                                      pts.ctypes.data_as(C.POINTER(C.c_int64)), ww.ctypes.data_as(C.POINTER(C.c_double)),
+                                                      int(t0), int(nrows)))
         self._nrcv, self._nrows_r = pts.shape[0], int(nrows)
 
     def get_traces(self):

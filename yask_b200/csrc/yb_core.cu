@@ -955,6 +955,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
         if (te1) cudaEventDestroy(te1);
     }
     if (s->halo && rc >= 0) rc = halo_finish(*s, st);   // the last exchange completes inside the run (and its timing)
+    if (s->halo && rc >= 0) rc = points_record_pending(*s, st);        // then the last step's weighted receivers
     YB_CUDA(cudaEventRecord(e1, st));
     return rc < 0 ? rc : 0;
 }

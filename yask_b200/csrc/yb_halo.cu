@@ -233,7 +233,7 @@ void halo_mark_dirty(Solution& s, int var) {
 }
 
 // Does var v need data from the neighbour in direction dir?  (L1-norm pruning + nonzero halo width.)
-static bool var_talks_to(const Var& v, const int dir[3]) {
+bool var_talks_to(const Var& v, const int dir[3]) {
     int l1 = abs(dir[0]) + abs(dir[1]) + abs(dir[2]);
     if (l1 > v.spec.l1_norm) return false;
     for (int k = 0; k < 3; k++) {
@@ -495,6 +495,9 @@ static bool other_dirty(const HaloState* h, int var, int slot) {
 // than the widest x halo from every x interface (no neighbour reads them).  A rank that owns a source nearer than that runs the
 // stage in the split form instead: the fused launch stores and publishes its boundary planes itself, before a source could enter.
 // Both forms advance the epoch once, so the choice is the rank's own.
+// Weighted receivers (yb_points.h) may read halo cells, which hold the neighbours' values of step u only once the step's last
+// exchange has arrived: the last stage defers them, and they are recorded right after that wait -- at the top of the next step's
+// first stage, or after halo_finish at the end of the run -- before the next step's first launch on this stream.
 // Slice recorders (yb_slices.h) only read: they record in the last stage, after the launch that computed the rank's last points
 // and that launch's points (fused: the launch; whole: the launch; split: the interior launch), on this stream, so before the next
 // step's first launch overwrites an in-place var.  They never change the form.
@@ -504,6 +507,7 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     HaloState* h = s.halo;
     if (!h->finalized) return set_error(YB_ESTATE, "multi-rank solution: halo peers were not connected (yb_halo_import/finalize)");
     if (int rc = halo_flush_wait(s, st)) return rc;
+    if (int rc = points_record_pending(s, st); rc < 0) return rc;       // the previous step's weighted receivers, halos now final
     const StageSpec& sp = s.spec.stages[stage];
     auto mark_outputs_dirty = [&]() {
         for (int vi : sp.outputs) h->dirty[vi][s.vars[vi].slot_of(t + sp.out_step_off)] = 1;

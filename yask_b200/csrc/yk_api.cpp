@@ -8,6 +8,7 @@
 #include "../include/yask_b200_points.hpp"
 #include "../include/yask_b200_slices.hpp"
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
@@ -860,6 +861,79 @@ idx_t yk_get_point_launches(yk_solution_ptr soln) {
     char v[64];
     chk(yb_get_option(b200(soln).h->s, "point_launches", v, sizeof v));
     return idx_t(atoll(v));
+}
+
+namespace {
+// n x k x ndd indices and n x k weights, flattened; every point must have the same k entries of ndd indices
+void flat_weighted(B200Solution& s, const std::vector<std::vector<idx_t_vec>>& idx, const std::vector<std::vector<double>>& w, const char* what,
+                   std::vector<int64_t>& pts, std::vector<double>& ws, size_t& k) {
+    const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
+    if (idx.size() != w.size())
+        fail(std::string(what) + ": " + std::to_string(idx.size()) + " index lists but " + std::to_string(w.size()) + " weight lists");
+    k = idx.empty() ? 0 : idx[0].size();
+    for (size_t i = 0; i < idx.size(); i++) {
+        if (idx[i].size() != k || w[i].size() != k)
+            fail(std::string(what) + ": point " + std::to_string(i) + " has " + std::to_string(idx[i].size()) + " entries and " +
+                 std::to_string(w[i].size()) + " weights; point 0 has " + std::to_string(k) + " entries");
+        for (size_t q = 0; q < k; q++) {
+            if (idx[i][q].size() != nd)
+                fail(std::string(what) + ": point " + std::to_string(i) + " entry " + std::to_string(q) + " has " + std::to_string(idx[i][q].size()) +
+                     " indices but the solution has " + std::to_string(nd) + " domain dims");
+            pts.insert(pts.end(), idx[i][q].begin(), idx[i][q].end());
+        }
+        ws.insert(ws.end(), w[i].begin(), w[i].end());
+    }
+}
+}  // namespace
+
+void yk_set_sources_weighted(yk_solution_ptr soln, const std::string& var, const std::vector<std::vector<idx_t_vec>>& idx,
+                             const std::vector<std::vector<double>>& w, idx_t t0, const std::vector<std::vector<double>>& amp) {
+    B200Solution& s = b200(soln);
+    std::vector<int64_t> pts;
+    std::vector<double> ws, flat;
+    size_t k = 0;
+    flat_weighted(s, idx, w, "weighted sources", pts, ws, k);
+    for (size_t r = 0; r < amp.size(); r++) {
+        if (amp[r].size() != idx.size())
+            fail("weighted sources: amplitude row " + std::to_string(r) + " has " + std::to_string(amp[r].size()) + " values for " +
+                 std::to_string(idx.size()) + " source(s)");
+        flat.insert(flat.end(), amp[r].begin(), amp[r].end());
+    }
+    chk(yb_solution_set_sources_weighted(s.h->s, var.c_str(), int64_t(idx.size()), int64_t(k), pts.data(), ws.data(), t0, int64_t(amp.size()),
+                                         flat.data()));
+}
+
+void yk_set_receivers_weighted(yk_solution_ptr soln, const std::string& var, const std::vector<std::vector<idx_t_vec>>& idx,
+                               const std::vector<std::vector<double>>& w, idx_t t0, idx_t nrows) {
+    B200Solution& s = b200(soln);
+    std::vector<int64_t> pts;
+    std::vector<double> ws;
+    size_t k = 0;
+    flat_weighted(s, idx, w, "weighted receivers", pts, ws, k);
+    chk(yb_solution_set_receivers_weighted(s.h->s, var.c_str(), int64_t(idx.size()), int64_t(k), pts.data(), ws.data(), t0, nrows));
+    s.point_rcv = idx_t(idx.size());
+    s.point_rows = nrows;
+}
+
+void yk_trilinear(const std::vector<std::vector<double>>& pos, std::vector<std::vector<idx_t_vec>>& idx, std::vector<std::vector<double>>& w) {
+    const size_t n = pos.size(), nd = n ? pos[0].size() : 0;
+    std::vector<double> flat;
+    for (size_t i = 0; i < n; i++) {
+        if (pos[i].size() != nd)
+            fail("trilinear: position " + std::to_string(i) + " has " + std::to_string(pos[i].size()) + " coordinates; position 0 has " + std::to_string(nd));
+        flat.insert(flat.end(), pos[i].begin(), pos[i].end());
+    }
+    const size_t k = size_t(1) << std::min<size_t>(nd, 3);
+    std::vector<int64_t> fi(n * k * nd);
+    std::vector<double> fw(n * k);
+    chk(yb_points_trilinear(int(nd), int64_t(n), flat.data(), fi.data(), fw.data()));
+    idx.assign(n, std::vector<idx_t_vec>(k, idx_t_vec(nd)));
+    w.assign(n, std::vector<double>(k));
+    for (size_t i = 0; i < n; i++)
+        for (size_t q = 0; q < k; q++) {
+            for (size_t d = 0; d < nd; d++) idx[i][q][d] = fi[(i * k + q) * nd + d];
+            w[i][q] = fw[i * k + q];
+        }
 }
 
 // ---- slice recorders (yask_b200_slices.hpp) ------------------------------------------------------------------------

@@ -294,6 +294,16 @@ PYBIND11_MODULE(yask_kernel, m) {
     }, py::arg("soln"), "(traces[row][receiver] as floats, owned[receiver])");
     m.def("yk_clear_points", &yk_clear_points, py::arg("soln"));
     m.def("yk_get_point_launches", &yk_get_point_launches, py::arg("soln"));
+    m.def("yk_set_sources_weighted", &yk_set_sources_weighted, py::arg("soln"), py::arg("var"), py::arg("idx"), py::arg("w"), py::arg("t0"),
+          py::arg("amp"));
+    m.def("yk_set_receivers_weighted", &yk_set_receivers_weighted, py::arg("soln"), py::arg("var"), py::arg("idx"), py::arg("w"), py::arg("t0"),
+          py::arg("nrows"));
+    m.def("yk_trilinear", [](const std::vector<std::vector<double>>& pos) {
+        std::vector<std::vector<idx_t_vec>> idx;
+        std::vector<std::vector<double>> w;
+        yk_trilinear(pos, idx, w);
+        return py::make_tuple(idx, w);
+    }, py::arg("pos"), "(idx[point][entry][dim], w[point][entry]) of the trilinear support of each position");
 
     // ---- slice recorders on the device (yask_b200_slices.hpp; not in the reference API) ----
     m.def("yk_add_slice", &yk_add_slice, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"), py::arg("t0"), py::arg("nrows"),

@@ -30,4 +30,16 @@ void yk_clear_points(yk_solution_ptr soln);
 // Point-kernel launches since prepare_solution().
 idx_t yk_get_point_launches(yk_solution_ptr soln);
 
+// Weighted sets: sources and receivers between grid points (yb_solution_set_sources_weighted in include/yask_b200.h).  idx[i][q]
+// is the q-th support point of point i (global domain indices) and w[i][q] its weight; every point has the same number of
+// entries.  Sources add w[i][q] * amp[u - t0][i] in (i, q) order; receiver j records the double sum of w[j][q] * var(u, idx[j][q])
+// rounded to the element type.  Each replaces the set of its kind.
+void yk_set_sources_weighted(yk_solution_ptr soln, const std::string& var, const std::vector<std::vector<idx_t_vec>>& idx,
+                             const std::vector<std::vector<double>>& w, idx_t t0, const std::vector<std::vector<double>>& amp);
+void yk_set_receivers_weighted(yk_solution_ptr soln, const std::string& var, const std::vector<std::vector<idx_t_vec>>& idx,
+                               const std::vector<std::vector<double>>& w, idx_t t0, idx_t nrows);
+// Trilinear support of real-valued positions in global index units (yb_points_trilinear): idx[i] gets 2^ndd points, w[i] their
+// weights, x varying slowest.
+void yk_trilinear(const std::vector<std::vector<double>>& pos, std::vector<std::vector<idx_t_vec>>& idx, std::vector<std::vector<double>>& w);
+
 }  // namespace yask
