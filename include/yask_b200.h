@@ -283,6 +283,30 @@ int yb_solution_add_slice(yb_solution* s, const char* var, const int64_t* first,
 int yb_solution_get_slice_frames(yb_solution* s, int64_t id, void* out, uint8_t* owned);
 int yb_solution_clear_slices(yb_solution* s);      /* remove every recorder and free its frames; ids restart at 0 */
 
+/* ---- slice injectors: boxes written into a var on the device inside run_solution() ----------------------------------
+ * The dual of a recorder, for plane-wave and areal sources, back-propagating a recorded plane, boundary replay and time-varying
+ * Dirichlet data.  It replaces the host loop run_solution(t, t); get_elements_in_slice(box, {u, first...}, {u, last...});
+ * box[::stride] = frame (or box[::stride] + frame); set_elements_in_slice(box) with one call, bit for bit.  The box (first, last,
+ * stride), the window (t0, every, nrows) and the var rules are those of yb_solution_add_slice.  `frames` holds nrows x the
+ * decimated box of the solution's element type, the last domain dim fastest; the call copies it.  Whenever a run has computed
+ * step u (u = t+1, or t-1 for a reverse solution), if u - t0 is a multiple of `every` and r = (u - t0) / every is in [0, nrows),
+ * then for every point pt of the decimated box:
+ *   YB_INJECT_SET: var(u, pt) = frame[r][pt];
+ *   YB_INJECT_ADD: var(u, pt) = T(var(u, pt) + frame[r][pt]), one add in the element type (add_to_element's rounding).
+ * Within step u, after all its stages: the injectors in id order (where two on one var overlap, the later id wins or adds last),
+ * then the sources, the receivers and the recorders, which so see the injection.  On a rank grid each rank writes its own part
+ * of the box, and the var must be written by the last stage (as for sources); neighbours receive the values through that stage's
+ * exchange.  Each rank keeps nrows x its own part on the device, allocated and uploaded at this call on a prepared solution
+ * (which synchronizes its stream), otherwise at prepare -- never in run_solution().  While any injector is set every run takes
+ * one step per launch (block_steps pairs resume once they are cleared); a fused-pair rank grid refuses them.  *id (0, 1, ...)
+ * names the injector; ids are separate from the recorders'.  Read-only options: slice_injector_groups, the launch groups in order
+ * (ids in a group separated by ',', groups by ';', e.g. "0,1;2": a group ends before an injector whose box meets that of an
+ * earlier member on the same var); slice_injector_launches, injecting launches since prepare (one per group with a row due). */
+enum { YB_INJECT_ADD = 0, YB_INJECT_SET = 1 };
+int yb_solution_add_slice_injector(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                   int64_t t0, int64_t every, int64_t nrows, int mode, const void* frames, int64_t* id);
+int yb_solution_clear_slice_injectors(yb_solution* s);   /* remove every injector and free its frames; ids restart at 0 */
+
 /* ---- multi-GPU halo exchange, one process per GPU (replaces exchange_halos, halo.cpp:80-491) --- */
 /* Each rank exports an opaque blob (CUDA IPC handles of its var storage + sync flags), the
  * launcher all-gathers the blobs (torch.distributed / MPI / files) and imports every

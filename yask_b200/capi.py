@@ -63,6 +63,7 @@ ABI_SYMBOLS = [
     "yb_get_stats", "yb_clear_stats", "yb_solution_set_sources", "yb_solution_set_receivers", "yb_solution_get_traces",
     "yb_solution_clear_points", "yb_solution_set_sources_weighted", "yb_solution_set_receivers_weighted", "yb_points_trilinear",
     "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
+    "yb_solution_add_slice_injector", "yb_solution_clear_slice_injectors",
     "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
@@ -139,6 +140,9 @@ def lib() -> C.CDLL:
         L.yb_solution_add_slice.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, C.POINTER(i64)]
         L.yb_solution_get_slice_frames.argtypes = [p, i64, p, C.POINTER(C.c_uint8)]
         L.yb_solution_clear_slices.argtypes = [p]
+        L.yb_solution_add_slice_injector.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, i32, p,
+                                                     C.POINTER(i64)]
+        L.yb_solution_clear_slice_injectors.argtypes = [p]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
         L.yb_halo_export.argtypes = [p, p, C.c_size_t]
         L.yb_halo_import.argtypes = [p, i64, p, C.c_size_t]
@@ -538,6 +542,41 @@ class Solution:
     def clear_slices(self):
         _chk(lib().yb_solution_clear_slices(self._h))
         self._slices = {}
+
+    # slice injectors (yb_solution_add_slice_injector / clear_slice_injectors)
+    INJECT_MODES = {"add": 0, "set": 1}        # YB_INJECT_ADD, YB_INJECT_SET
+
+    def add_slice_injector(self, var: str, first, last, t0: int, frames, stride=None, every: int = 1, mode: str = "add") -> int:
+        """After every step u a run computes with u - t0 a multiple of `every` and r = (u - t0) // every below len(frames), set
+        (mode "set") or add frames[r] to (mode "add", one add in the element type) var(u) at the box first[d], first[d] +
+        stride[d], ... <= last[d] (global domain indices).  frames: (nrows, *box_shape); a real array of another dtype is rounded
+        to the element type.  The frames are copied.  Returns the injector's id."""
+        nd = len(self.get_domain_dim_names())
+        f, l = np.atleast_1d(np.asarray(first, np.int64)), np.atleast_1d(np.asarray(last, np.int64))
+        st = np.ones(nd, np.int64) if stride is None else np.atleast_1d(np.asarray(stride, np.int64))
+        for what, a in (("first", f), ("last", l), ("stride", st)):
+            if a.shape != (nd,):
+                raise YaskError(-1, f"slice injector: {what} needs {nd} domain index(es) ({', '.join(self.get_domain_dim_names())}), "
+                                    f"got {a.tolist()}")
+        if mode not in self.INJECT_MODES:
+            raise YaskError(-1, f"slice injector: unknown mode {mode!r} (expected 'add' or 'set')")
+        fr = np.asarray(frames)
+        if np.iscomplexobj(fr) or not (np.issubdtype(fr.dtype, np.floating) or np.issubdtype(fr.dtype, np.integer)):
+            raise YaskError(-1, f"slice injector: frames of dtype {fr.dtype} are not real numbers")
+        box = tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1)
+        # an empty box or a stride below 1 is left to the engine, which names it
+        if (l >= f).all() and (st >= 1).all() and (fr.ndim != nd + 1 or tuple(fr.shape[1:]) != box):
+            raise YaskError(-1, f"slice injector: frames of shape {fr.shape} do not match the decimated box: expected "
+                                f"(nrows, {', '.join(str(b) for b in box)})")
+        fr = np.ascontiguousarray(fr, dtype=np.float32 if self.get_element_bytes() == 4 else np.float64)
+        rid = C.c_int64(-1)
+        _chk(lib().yb_solution_add_slice_injector(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                  int(t0), int(every), fr.shape[0] if fr.ndim else 0, self.INJECT_MODES[mode], fr.ctypes.data,
+                                                  C.byref(rid)))
+        return rid.value
+
+    def clear_slice_injectors(self):
+        _chk(lib().yb_solution_clear_slice_injectors(self._h))
 
     def is_prepared(self) -> bool:
         return bool(lib().yb_solution_is_prepared(self._h))

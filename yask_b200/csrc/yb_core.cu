@@ -43,6 +43,7 @@ Solution::~Solution() {
     }
     points_free(points);     // device tables are released on `device`, selected above
     slices_free(slices);
+    slices_free(injectors);
 }
 
 static int check_dim(const Solution* s, int dim) {
@@ -405,7 +406,8 @@ int yb_set_option(yb_solution* s_, const char* key, const char* value) {
     } else if (k == "auto_tune") {
         s->tuner = Solution::InRunTuner();
         s->tuner.enabled = atoi(value) != 0;
-    } else if (k == "point_launches" || k == "point_groups" || k == "slice_launches") {
+    } else if (k == "point_launches" || k == "point_groups" || k == "slice_launches" || k == "slice_injector_groups" ||
+               k == "slice_injector_launches") {
         return set_error(YB_EINVAL, "option '%s' is read-only", key);
     } else if (k == "overlap_comms" || k == "min_exterior" || k == "fused_halo" || k == "dma_halo") {
         // consumed by the halo engine at run time
@@ -423,6 +425,8 @@ int yb_get_option(const yb_solution* s_, const char* key, char* value, size_t n)
     else if (std::string(key) == "point_launches") v = std::to_string(s->points ? s->points->launches : 0);   // read-only
     else if (std::string(key) == "point_groups") v = points_groups_text(*s);                                    // read-only
     else if (std::string(key) == "slice_launches") v = std::to_string(s->slices ? s->slices->launches : 0);   // read-only
+    else if (std::string(key) == "slice_injector_groups") v = slice_injector_groups_text(*s);                   // read-only
+    else if (std::string(key) == "slice_injector_launches") v = std::to_string(s->injectors ? s->injectors->launches : 0);   // read-only
     else if (!s->engine->get_option(*s, key, v)) {
         auto it = s->options.find(key);
         if (it == s->options.end()) return set_error(YB_EINVAL, "unknown option '%s'", key);
@@ -458,7 +462,7 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     if (int rc = s->engine->check_geometry(*s)) return rc;
     if (points_active(*s))
         if (int rc = points_plan(*s)) return rc;          // point sets given before the geometry are checked now
-    return slices_plan(*s);                               // and so are slice recorders
+    return slices_plan(*s);                               // and so are slice recorders and injectors
 }
 
 int yb_solution_prepare(yb_solution* s_, int device) {
@@ -502,8 +506,9 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (s->multi_rank()) {
         if (int rc = halo_prepare(*s)) return rc;
     }
-    if (int rc = slices_prepare(*s)) return rc;       // frames of the recorders added before prepare
+    if (int rc = slices_prepare(*s)) return rc;       // frames of the recorders and injectors added before prepare
     if (s->slices) s->slices->launches = 0;
+    if (s->injectors) s->injectors->launches = 0;
     YB_CUDA(cudaStreamSynchronize(s->stream()));
     s->prepared = true;
     memset(&s->stats, 0, sizeof s->stats);
@@ -877,10 +882,11 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward run goes through the engine's fused launch, `fs` steps
     // at a time; what is left over (and every other kind of run) takes the one-step path below.  A rank grid fuses steps only
     // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.  Point sources
-    // enter between two steps, and slice recorders read a step a pair would never store, so a solution with points or recorders
-    // runs one step per launch (both are refused on a rank grid in the fused mode).
+    // and slice injectors enter between two steps, and slice recorders read a step a pair would never store, so a solution with
+    // any of them runs one step per launch (all are refused on a rank grid in the fused mode).
     int64_t t_first = first_step;
-    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s) && !slices_active(*s)) ? s->engine->fused_steps(*s) : 1;
+    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s) && !slices_active(*s) && !slice_injectors_active(*s))
+                       ? s->engine->fused_steps(*s) : 1;
     if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
         const bool ends_run = t_first + fs - 1 == last_step;
@@ -926,7 +932,9 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
             s->stats.est_fp_ops_done += sp.fp_ops * pts;
             for (int vi : sp.outputs) s->vars[vi].update_valid_step(t + sp.out_step_off);
         }
-        // sources and receivers of the step just computed (a rank grid applies them inside its last stage, halo_run_stage)
+        // injectors, then sources and receivers of the step just computed (a rank grid applies them inside its last stage,
+        // halo_run_stage)
+        if (rc >= 0 && !s->halo) rc = slice_injectors_launch(*s, t, PTS_ALL, whole, st);
         if (rc >= 0 && !s->halo) rc = points_launch(*s, t, PTS_ALL, whole, st);
         // then the slice recorders, before the next step's first launch can overwrite an in-place var (halo_run_stage on a grid)
         if (rc >= 0 && !s->halo) rc = slices_launch(*s, t, st);

@@ -221,6 +221,8 @@ struct Solution {
     PointsState* points = nullptr;   // owned; freed by points_free()
     // slice recorders (yb_slices.h)
     SlicesState* slices = nullptr;   // owned; freed by slices_free()
+    // slice injectors (yb_slices.h)
+    SlicesState* injectors = nullptr;   // owned; freed by slices_free()
     // Fused halo stores (set by the halo layer before a stage launch, consumed by an engine that can store its
     // boundary planes straight into the x neighbours' halo cells): element (0,0,0)-relative base pointers of the
     // OUTPUT var's step slot in the lower / upper x neighbour, or null.  The engine sets `used` if it honoured them.

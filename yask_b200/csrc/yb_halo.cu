@@ -498,9 +498,22 @@ static bool other_dirty(const HaloState* h, int var, int slot) {
 // Weighted receivers (yb_points.h) may read halo cells, which hold the neighbours' values of step u only once the step's last
 // exchange has arrived: the last stage defers them, and they are recorded right after that wait -- at the top of the next step's
 // first stage, or after halo_finish at the end of the run -- before the next step's first launch on this stream.
+// Slice injectors (yb_slices.h) write the last stage's output like sources, just before them and in the same places; an injector
+// row whose owned part reaches within the widest x halo of an x interface with a neighbour turns the fused form into the split
+// form, as a source there does (writes_near_x_interface).  The split form injects the points outside the interior before the
+// pushes and the rest after the interior launch, so every point is written once and before the exchange that publishes it.
 // Slice recorders (yb_slices.h) only read: they record in the last stage, after the launch that computed the rank's last points
 // and that launch's points (fused: the launch; whole: the launch; split: the interior launch), on this stream, so before the next
 // step's first launch overwrites an in-place var.  They never change the form.
+// Does this rank write at step t, after the last stage's launch, within w planes of an x interface with a neighbour rank (point
+// sources, slice injectors)?  Such a write must come before the boundary planes are published, which the fused x launch does itself.
+static bool writes_near_x_interface(const Solution& s, int64_t t, int64_t w) {
+    const bool lo = s.rank_index[0] > 0, hi = s.rank_index[0] < s.num_ranks[0] - 1;
+    auto near = [&](int64_t x0, int64_t x1) { return (lo && x0 < w) || (hi && x1 >= s.rank_size[0] - w); };
+    int64_t x0 = 0, x1 = 0;
+    return (points_source_x_range(s, t, x0, x1) && near(x0, x1)) || (slice_injectors_x_range(s, t, x0, x1) && near(x0, x1));
+}
+
 int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     Box whole;
     for (int d = 0; d < 3; d++) { whole.b[d] = 0; whole.e[d] = d < s.ndd ? s.rank_size[d] : 1; }
@@ -514,14 +527,20 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
     };
     auto opt_off = [&](const char* key) { auto it = s.options.find(key); return it != s.options.end() && it->second == "0"; };
     const bool overlap = !opt_off("overlap_comms");
-    const bool points = stage + 1 == int(s.spec.stages.size()) && points_active(s);
-    auto apply_points = [&](int sel, const Box& interior) { return points ? points_launch(s, t, sel, interior, st) : 0; };
     const bool last_stage = stage + 1 == int(s.spec.stages.size());
+    // the last stage's writes after its launch: injectors first, then sources (and the receivers of the points kernel)
+    auto apply_points = [&](int sel, const Box& interior) {
+        if (!last_stage) return 0;
+        const int a = slice_injectors_launch(s, t, sel, interior, st);
+        if (a < 0) return a;
+        const int b = points_launch(s, t, sel, interior, st);
+        return b < 0 ? b : a + b;
+    };
     auto record_slices = [&]() { return last_stage ? slices_launch(s, t, st) : 0; };
     int64_t wx = 0;         // widest x halo: the planes of an x interface the neighbour reads
     for (auto& v : s.vars)
         if (const Dim* dx = v.domain_dim(0)) wx = std::max({wx, dx->spec.halo_l, dx->spec.halo_r});
-    const bool fused_ok = !opt_off("fused_halo") && !(points && points_source_near_x_interface(s, t, wx));
+    const bool fused_ok = !opt_off("fused_halo") && !(last_stage && writes_near_x_interface(s, t, wx));
 
     // ---- fused path -----------------------------------------------------------------------------------------
     s.fused_x = Solution::FusedX();

@@ -541,17 +541,17 @@ std::string points_groups_text(const Solution& s) {
     return out;
 }
 
-bool points_source_near_x_interface(const Solution& s, int64_t t, int64_t w) {
+bool points_source_x_range(const Solution& s, int64_t t, int64_t& x0, int64_t& x1) {
     if (!points_active(s) || !s.points->src.set) return false;
     const PointsState& p = *s.points;
     const int64_t row = t + p.src.step_off - p.src.t0;
-    if (row < 0 || row >= p.src.nrows) return false;
-    const bool lo = s.rank_index[0] > 0, hi = s.rank_index[0] < s.num_ranks[0] - 1;
-    for (size_t g = 0; g < p.plan.grp_off.size(); g++) {
-        const long long x = p.plan.grp_loc[3 * g];
-        if ((lo && x < w) || (hi && x >= s.rank_size[0] - w)) return true;
+    if (row < 0 || row >= p.src.nrows || p.plan.grp_off.empty()) return false;
+    x0 = x1 = p.plan.grp_loc[0];
+    for (size_t g = 1; g < p.plan.grp_off.size(); g++) {
+        x0 = std::min<int64_t>(x0, p.plan.grp_loc[3 * g]);
+        x1 = std::max<int64_t>(x1, p.plan.grp_loc[3 * g]);
     }
-    return false;
+    return true;
 }
 
 }  // namespace yb

@@ -81,7 +81,7 @@ int points_record_pending(Solution& s, cudaStream_t st);
 // comma-separated list indices of the sources it adds, in the order it adds them (e.g. "0,2;1"); a weighted set writes each
 // entry as source/support entry (e.g. "0/3,2/0;1/0")
 std::string points_groups_text(const Solution& s);
-// Does this rank apply a source at step t within `w` planes of an x interface with a neighbour rank?
-bool points_source_near_x_interface(const Solution& s, int64_t t, int64_t w);
+// rank-local x range [x0, x1] of the sources this rank applies at step t; false when it applies none
+bool points_source_x_range(const Solution& s, int64_t t, int64_t& x0, int64_t& x1);
 
 }  // namespace yb

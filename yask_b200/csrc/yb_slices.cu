@@ -1,6 +1,8 @@
 // Slice recorders on the device (yb_slices.h): receiver planes, decimated snapshots and field dumps every k steps, recorded
 // inside run_solution() by one many-CTA launch per step, instead of the reference API loop run_solution(t, t) /
-// get_elements_in_slice, which pays a synchronous device-to-host copy per frame and loses the temporal tile's pairs.
+// get_elements_in_slice, which pays a synchronous device-to-host copy per frame and loses the temporal tile's pairs.  Slice
+// injectors write boxes back the same way (plane-wave and areal sources, boundary replay, time-varying Dirichlet data), instead of
+// the loop run_solution(t, t) / get_elements_in_slice / set_elements_in_slice.
 #include <stdio.h>
 #include <string.h>
 
@@ -25,6 +27,10 @@ struct SliceDesc {
     long long t0, every, nrows;
     BoxDev box;                     // this rank's part: element offset of its first point, decimated strides
     char* frames;                   // nrows x box.total elements
+    // injectors: YB_INJECT_ADD / SET, and the rank-local coordinates of the first owned point and their step per box index
+    // (dims right-aligned as in box), which the split form's selection tests against the interior box
+    int mode;
+    long long loc0[4], lstep[4];
 };
 
 __host__ __device__ __forceinline__ bool row_due(long long u, long long t0, long long every, long long nrows, long long& row) {
@@ -53,11 +59,52 @@ __global__ void __launch_bounds__(256) slices_kernel(const SliceDesc* __restrict
     }
 }
 
+// the rounding of add_to_element: one add in the element type
+__device__ __forceinline__ float add_elem(float v, float a) { return __fadd_rn(v, a); }
+__device__ __forceinline__ double add_elem(double v, double a) { return __dadd_rn(v, a); }
+
+// which points of one injecting launch: PTS_ALL, or those outside (PTS_EXTERIOR) or inside (PTS_INTERIOR) the rank-local box
+struct InjectSel {
+    int sel;
+    long long ib[4], ie[4];         // right-aligned like BoxDev
+};
+
+// The dual of slices_kernel, with its layout: blockIdx.y walks the injectors table[first .. first + n) (one launch group, so no
+// two of them write one element), blockIdx.x and the threads the dense points of one, the unit-stride dim fastest; the frame row
+// is read contiguously.  Each point belongs to one thread: no atomics.
+template <typename T>
+__global__ void __launch_bounds__(256) slice_injectors_kernel(const SliceDesc* __restrict__ table, int first, int n, long long t, InjectSel q) {
+    for (int r = first + blockIdx.y; r < first + n; r += gridDim.y) {
+        const SliceDesc& d = table[r];
+        const long long u = t + d.step_off;
+        long long row;
+        if (!row_due(u, d.t0, d.every, d.nrows, row)) continue;
+        const BoxDev b = d.box;
+        long long slot = u % d.alloc;
+        slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
+        T* __restrict__ dst = reinterpret_cast<T*>(const_cast<char*>(d.var_base) + slot * d.slot_bytes);
+        const T* __restrict__ src = reinterpret_cast<const T*>(d.frames) + row * b.total;
+        const bool set = d.mode == YB_INJECT_SET;
+        long long coord[4];
+        for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) {
+            const long long o = box_offset(b, i, coord);
+            if (q.sel != PTS_ALL) {
+                bool in = true;
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const long long c = d.loc0[k] + coord[k] * d.lstep[k];
+                    in = in && c >= q.ib[k] && c < q.ie[k];
+                }
+                if (in != (q.sel == PTS_INTERIOR)) continue;
+            }
+            dst[o] = set ? src[i] : add_elem(dst[o], src[i]);
+        }
+    }
+}
+
 // The x grid is a grid-stride cap: 8 CTAs per SM is two waves at the 4 CTAs of 256 threads per SM that the kernel's 56
 // registers allow.  y: the hardware limit of gridDim.y; more recorders are walked by the y loop.
 constexpr int CTAS_PER_SM = 8, MAX_GRID_Y = 65535;
-
-const char* const WHAT = "slice";
 
 void release(SliceRec& r) {
     if (r.d_frames) cudaFree(r.d_frames);
@@ -66,15 +113,32 @@ void release(SliceRec& r) {
     r.uploaded_base = nullptr;
 }
 
-// this rank's part of one recorder; refuses a box outside the overall domain
-int plan_one(const Solution& s, SliceRec& r) {
+SlicesState* new_state(bool inject) {
+    SlicesState* p = new SlicesState();
+    p->inject = inject;
+    p->what = inject ? "slice injector" : "slice";
+    return p;
+}
+
+bool active(const SlicesState* p) { return p && !p->recs.empty(); }
+
+// this rank's part of one recorder or injector; refuses a box outside the overall domain, and on a rank grid an injector into a
+// var the last stage does not write (it must land before that stage's exchange, as a source does)
+int plan_one(const Solution& s, const SlicesState& p, SliceRec& r) {
     const Var& v = s.vars[r.var];
+    if (p.inject && s.multi_rank()) {
+        bool last = false;
+        for (int o : s.spec.stages.back().outputs) last = last || o == r.var;
+        if (!last)
+            return set_error(YB_EUNSUPPORTED, "%s: on a rank grid the var '%s' must be written by the last stage of '%s'", p.what,
+                             v.spec.name.c_str(), s.spec.name.c_str());
+    }
     r.own_off = 0;
     r.own_elems = 1;
     for (int k = 0; k < s.ndd; k++) {
         if (r.first[k] < 0 || r.last[k] >= s.overall_size[k])
             return set_error(YB_ERANGE, "%s: box [%lld, %lld] in dim '%s' is outside the overall domain [0,%lld) (halo and pad cells are refused)",
-                             WHAT, (long long)r.first[k], (long long)r.last[k], s.spec.domain_dims[k].c_str(), (long long)s.overall_size[k]);
+                             p.what, (long long)r.first[k], (long long)r.last[k], s.spec.domain_dims[k].c_str(), (long long)s.overall_size[k]);
         // owned decimated indices: first + k * stride inside [lo, hi]; the phase comes from the global first
         const int64_t lo = s.rank_offset[k], hi = lo + s.rank_size[k] - 1, st = r.stride[k];
         const int64_t k0 = r.first[k] >= lo ? 0 : (lo - r.first[k] + st - 1) / st;
@@ -88,6 +152,9 @@ int plan_one(const Solution& s, SliceRec& r) {
     return 0;
 }
 
+// rank-local coordinate of the first owned point in domain dim k (the last one is that + (own_n[k] - 1) * stride[k])
+int64_t own_loc0(const Solution& s, const SliceRec& r, int k) { return r.first[k] + r.own_k0[k] * r.stride[k] - s.rank_offset[k]; }
+
 SliceDesc describe(const Solution& s, const SliceRec& r) {
     const Var& v = s.vars[r.var];
     SliceDesc d{};
@@ -100,10 +167,13 @@ SliceDesc describe(const Solution& s, const SliceRec& r) {
     d.box.nd = s.ndd;
     d.box.off = r.own_off;
     d.box.total = r.own_elems;
-    for (int i = 0; i < 4; i++) { d.box.n[i] = 1; d.box.vs[i] = 0; }
+    d.mode = r.mode;
+    for (int i = 0; i < 4; i++) { d.box.n[i] = 1; d.box.vs[i] = 0; d.loc0[i] = 0; d.lstep[i] = 0; }
     for (int k = 0; k < s.ndd; k++) {
         d.box.n[4 - s.ndd + k] = r.own_n[k];
         d.box.vs[4 - s.ndd + k] = v.domain_dim(k)->stride * r.stride[k];
+        d.loc0[4 - s.ndd + k] = own_loc0(s, r, k);
+        d.lstep[4 - s.ndd + k] = r.stride[k];
     }
     d.frames = static_cast<char*>(r.d_frames);
     return d;
@@ -111,24 +181,50 @@ SliceDesc describe(const Solution& s, const SliceRec& r) {
 
 size_t frame_bytes(const Solution& s, const SliceRec& r) { return size_t(r.nrows) * size_t(r.own_elems) * s.spec.elem_bytes; }
 
-int alloc_frames(const Solution& s, SliceRec& r) {
+// The owned part of `rows` rows of the whole decimated box as contiguous runs of the last dim: f(element index of the run in
+// rows x the whole box, its index in rows x the owned part, length).
+template <typename F>
+void owned_runs(const Solution& s, const SliceRec& r, int64_t rows, F f) {
+    int64_t cnt[3] = {1, 1, 1}, k0[3] = {0, 0, 0}, kn[3] = {1, 1, 1};
+    for (int k = 0; k < s.ndd; k++) { cnt[k] = r.count[k]; k0[k] = r.own_k0[k]; kn[k] = r.own_n[k]; }
+    size_t dense = 0;
+    for (int64_t row = 0; row < rows; row++)
+        for (int64_t a = 0; a < kn[0]; a++)
+            for (int64_t b = 0; b < kn[1]; b++, dense += size_t(kn[2]))
+                f(((size_t(row) * cnt[0] + k0[0] + a) * cnt[1] + k0[1] + b) * cnt[2] + k0[2], dense, size_t(kn[2]));
+}
+
+// Recorders: zeroed frames.  Injectors: this rank's part of the caller's frames, after which the host copy is dropped (the
+// geometry is fixed once a solution is prepared).
+int alloc_frames(const Solution& s, const SlicesState& p, SliceRec& r) {
     const size_t bytes = frame_bytes(s, r);
-    if (!bytes || r.d_frames) return 0;
+    if (r.d_frames) return 0;
+    if (!bytes) {
+        std::vector<char>().swap(r.host_frames);
+        return 0;
+    }
     cudaError_t e = cudaMalloc(&r.d_frames, bytes);
     if (e != cudaSuccess) {
         (void)cudaGetLastError();
         r.d_frames = nullptr;
-        return set_error(YB_ENOMEM, "%s: cannot allocate %zu bytes of frames (%lld rows x %lld owned points) on device %d: %s", WHAT, bytes,
+        return set_error(YB_ENOMEM, "%s: cannot allocate %zu bytes of frames (%lld rows x %lld owned points) on device %d: %s", p.what, bytes,
                          (long long)r.nrows, (long long)r.own_elems, s.device, cudaGetErrorString(e));
     }
-    YB_CUDA(cudaMemset(r.d_frames, 0, bytes));
+    if (!p.inject) {
+        YB_CUDA(cudaMemset(r.d_frames, 0, bytes));
+        return 0;
+    }
+    const size_t eb = size_t(s.spec.elem_bytes);
+    std::vector<char> dense(bytes);
+    owned_runs(s, r, r.nrows, [&](size_t whole, size_t own, size_t n) { memcpy(dense.data() + own * eb, r.host_frames.data() + whole * eb, n * eb); });
+    YB_CUDA(cudaMemcpy(r.d_frames, dense.data(), bytes, cudaMemcpyHostToDevice));
+    std::vector<char>().swap(r.host_frames);
     return 0;
 }
 
 // (re)write the device table; the caller has synchronized the stream.  The table is reallocated only when recorders were
 // added (add_slice, prepare), so the refresh at the start of a run copies and never allocates.
-int upload_table(Solution& s) {
-    SlicesState& p = *s.slices;
+int upload_table(Solution& s, SlicesState& p) {
     std::vector<SliceDesc> t;
     for (auto& r : p.recs) {
         t.push_back(describe(s, r));
@@ -148,6 +244,72 @@ int upload_table(Solution& s) {
     return 0;
 }
 
+// Launch groups of the injectors, in id order: a new group starts at injector j when the bounding box of its decimated box meets
+// that of an earlier member of the current group on the same var, so that no two injectors of one launch write one element and
+// the later id still applies last.  Global boxes only: every rank forms the same groups.
+void plan_groups(SlicesState& p) {
+    p.group_first.assign(1, 0);
+    for (size_t j = 0; j < p.recs.size(); j++) {
+        const SliceRec& b = p.recs[j];
+        bool meets = false;
+        for (size_t m = size_t(p.group_first.back()); m < j && !meets; m++) {
+            const SliceRec& a = p.recs[m];
+            meets = a.var == b.var;
+            for (int k = 0; k < 3 && meets; k++)
+                meets = a.first[k] <= b.first[k] + (b.count[k] - 1) * b.stride[k] && b.first[k] <= a.first[k] + (a.count[k] - 1) * a.stride[k];
+        }
+        if (meets) p.group_first.push_back(int(j));
+    }
+    if (!p.recs.empty()) p.group_first.push_back(int(p.recs.size()));
+}
+
+int check_mode(const Solution& s, const SlicesState& p) {
+    if (fused_pair_rank_grid(s))
+        return set_error(YB_EUNSUPPORTED, "%s are not supported on a rank grid in fused-pair mode (block_steps=2 with "
+                                          "mega_block_steps=2): its halos are exchanged once per pair of steps, and the state after the first "
+                                          "step of a pair is never stored", p.inject ? "slice injectors" : "slice recorders");
+    return 0;
+}
+
+int plan_state(Solution& s, SlicesState* p) {
+    if (!active(p)) return 0;
+    if (int rc = check_mode(s, *p)) return rc;
+    for (auto& r : p->recs)
+        if (int rc = plan_one(s, *p, r)) return rc;
+    return 0;
+}
+
+int prepare_state(Solution& s, SlicesState* p) {
+    if (!active(p)) return 0;
+    if (int rc = plan_state(s, p)) return rc;
+    for (auto& r : p->recs)
+        if (int rc = alloc_frames(s, *p, r)) return rc;
+    return upload_table(s, *p);
+}
+
+int begin_run_state(Solution& s, SlicesState* p) {
+    if (!active(p)) return 0;
+    if (int rc = check_mode(s, *p)) return rc;
+    bool moved = false;
+    for (auto& r : p->recs) moved = moved || r.uploaded_bias != s.vars[r.var].slot_bias || r.uploaded_base != s.vars[r.var].dev;
+    if (!moved) return 0;
+    YB_CUDA(cudaStreamSynchronize(s.stream()));
+    return upload_table(s, *p);
+}
+
+// Does an injecting launch with selection `sel` have any of r's owned points to write?  The owned part's rank-local bounding box
+// against the interior box (a stride may step over the interior: then the launch finds nothing, which is harmless).
+bool selects(const Solution& s, const SliceRec& r, int sel, const Box& interior) {
+    if (sel == PTS_ALL) return true;
+    bool inside = true, meets = true;
+    for (int k = 0; k < s.ndd; k++) {
+        const int64_t lo = own_loc0(s, r, k), hi = lo + (r.own_n[k] - 1) * r.stride[k];
+        inside = inside && lo >= interior.b[k] && hi < interior.e[k];
+        meets = meets && hi >= interior.b[k] && lo < interior.e[k];
+    }
+    return sel == PTS_INTERIOR ? meets : !inside;
+}
+
 }  // namespace
 
 void slices_free(SlicesState* p) {
@@ -160,42 +322,27 @@ void slices_free(SlicesState* p) {
 void slices_preload() {
     preload_kernel((const void*)slices_kernel<float>);
     preload_kernel((const void*)slices_kernel<double>);
+    preload_kernel((const void*)slice_injectors_kernel<float>);
+    preload_kernel((const void*)slice_injectors_kernel<double>);
 }
 
-bool slices_active(const Solution& s) { return s.slices && !s.slices->recs.empty(); }
+bool slices_active(const Solution& s) { return active(s.slices); }
 
-static int check_mode(const Solution& s) {
-    if (fused_pair_rank_grid(s))
-        return set_error(YB_EUNSUPPORTED, "slice recorders are not supported on a rank grid in fused-pair mode (block_steps=2 with "
-                                          "mega_block_steps=2): its halos are exchanged once per pair of steps, and the state after the first "
-                                          "step of a pair is never stored");
-    return 0;
-}
+bool slice_injectors_active(const Solution& s) { return active(s.injectors); }
 
 int slices_plan(Solution& s) {
-    if (!slices_active(s)) return 0;
-    if (int rc = check_mode(s)) return rc;
-    for (auto& r : s.slices->recs)
-        if (int rc = plan_one(s, r)) return rc;
-    return 0;
+    if (int rc = plan_state(s, s.slices)) return rc;
+    return plan_state(s, s.injectors);
 }
 
 int slices_prepare(Solution& s) {
-    if (!slices_active(s)) return 0;
-    if (int rc = slices_plan(s)) return rc;
-    for (auto& r : s.slices->recs)
-        if (int rc = alloc_frames(s, r)) return rc;
-    return upload_table(s);
+    if (int rc = prepare_state(s, s.slices)) return rc;
+    return prepare_state(s, s.injectors);
 }
 
 int slices_begin_run(Solution& s) {
-    if (!slices_active(s)) return 0;
-    if (int rc = check_mode(s)) return rc;
-    bool moved = false;
-    for (auto& r : s.slices->recs) moved = moved || r.uploaded_bias != s.vars[r.var].slot_bias || r.uploaded_base != s.vars[r.var].dev;
-    if (!moved) return 0;
-    YB_CUDA(cudaStreamSynchronize(s.stream()));
-    return upload_table(s);
+    if (int rc = begin_run_state(s, s.slices)) return rc;
+    return begin_run_state(s, s.injectors);
 }
 
 int slices_launch(Solution& s, int64_t t, cudaStream_t st) {
@@ -216,65 +363,165 @@ int slices_launch(Solution& s, int64_t t, cudaStream_t st) {
     return 1;
 }
 
+int slice_injectors_launch(Solution& s, int64_t t, int sel, const Box& interior, cudaStream_t st) {
+    if (!slice_injectors_active(s)) return 0;
+    SlicesState& p = *s.injectors;
+    InjectSel q{};
+    q.sel = sel;
+    for (int i = 0; i < 4; i++) { q.ib[i] = 0; q.ie[i] = 1; }
+    for (int k = 0; k < s.ndd; k++) { q.ib[4 - s.ndd + k] = interior.b[k]; q.ie[4 - s.ndd + k] = interior.e[k]; }
+    const SliceDesc* table = static_cast<const SliceDesc*>(p.d_table);
+    int launched = 0;
+    for (size_t g = 0; g + 1 < p.group_first.size(); g++) {
+        const int g0 = p.group_first[g], g1 = p.group_first[g + 1];
+        int64_t most = 0;
+        for (int j = g0; j < g1; j++) {
+            const SliceRec& r = p.recs[size_t(j)];
+            long long row;
+            if (r.own_elems && row_due(t + r.step_off, r.t0, r.every, r.nrows, row) && selects(s, r, sel, interior)) most = std::max(most, r.own_elems);
+        }
+        if (!most) continue;
+        const dim3 grid(unsigned(std::min<int64_t>((most + 255) / 256, int64_t(p.num_sms) * CTAS_PER_SM)), unsigned(std::min(g1 - g0, MAX_GRID_Y)));
+        if (s.spec.elem_bytes == 4) slice_injectors_kernel<float><<<grid, 256, 0, st>>>(table, g0, g1 - g0, t, q);
+        else slice_injectors_kernel<double><<<grid, 256, 0, st>>>(table, g0, g1 - g0, t, q);
+        YB_CUDA(cudaGetLastError());
+        p.launches++;
+        launched++;
+    }
+    return launched;
+}
+
+bool slice_injectors_x_range(const Solution& s, int64_t t, int64_t& x0, int64_t& x1) {
+    if (!slice_injectors_active(s)) return false;
+    bool any = false;
+    for (const SliceRec& r : s.injectors->recs) {
+        long long row;
+        if (!r.own_elems || !row_due(t + r.step_off, r.t0, r.every, r.nrows, row)) continue;
+        const int64_t lo = own_loc0(s, r, 0), hi = lo + (r.own_n[0] - 1) * r.stride[0];
+        x0 = any ? std::min(x0, lo) : lo;
+        x1 = any ? std::max(x1, hi) : hi;
+        any = true;
+    }
+    return any;
+}
+
+std::string slice_injector_groups_text(const Solution& s) {
+    std::string out;
+    if (!slice_injectors_active(s)) return out;
+    const std::vector<int>& gf = s.injectors->group_first;
+    for (size_t g = 0; g + 1 < gf.size(); g++) {
+        if (g) out += ';';
+        for (int j = gf[g]; j < gf[g + 1]; j++) out += (j > gf[g] ? "," : "") + std::to_string(j);
+    }
+    return out;
+}
+
 }  // namespace yb
 
 using namespace yb;
 
-extern "C" {
-
 #define SOL(s) reinterpret_cast<Solution*>(s)
 
-int yb_solution_add_slice(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
-                          int64_t t0, int64_t every, int64_t nrows, int64_t* id) {
-    Solution* s = SOL(s_);
-    if (!s) return set_error(YB_EINVAL, "null solution");
-    if (!first || !last) return set_error(YB_EINVAL, "%s: null box", WHAT);
-    SliceRec r;
-    if (int rc = point_var(*s, WHAT, var, r.var, r.step_off)) return rc;
+// The checks shared by recorders and injectors: the var, the box, the window and a 64-bit byte count of the frames of the whole
+// box (which bound every rank's share).  Fills r up to the window; `bytes`: nrows x the decimated box in bytes.
+static int new_rec(Solution* s, const char* what, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                   int64_t t0, int64_t every, int64_t nrows, SliceRec& r, int64_t& bytes) {
+    if (!first || !last) return set_error(YB_EINVAL, "%s: null box", what);
+    if (int rc = point_var(*s, what, var, r.var, r.step_off)) return rc;
     for (int k = 0; k < s->ndd; k++) {
         const char* dn = s->spec.domain_dims[k].c_str();
         r.first[k] = first[k];
         r.last[k] = last[k];
         r.stride[k] = stride ? stride[k] : 1;
         if (r.first[k] > r.last[k])
-            return set_error(YB_EINVAL, "%s: first index %lld is past last index %lld in dim '%s'", WHAT, (long long)r.first[k], (long long)r.last[k], dn);
-        if (r.stride[k] < 1) return set_error(YB_EINVAL, "%s: stride %lld in dim '%s' is less than 1", WHAT, (long long)r.stride[k], dn);
+            return set_error(YB_EINVAL, "%s: first index %lld is past last index %lld in dim '%s'", what, (long long)r.first[k], (long long)r.last[k], dn);
+        if (r.stride[k] < 1) return set_error(YB_EINVAL, "%s: stride %lld in dim '%s' is less than 1", what, (long long)r.stride[k], dn);
         r.count[k] = (r.last[k] - r.first[k]) / r.stride[k] + 1;
     }
-    if (every < 1) return set_error(YB_EINVAL, "%s: every = %lld is less than 1", WHAT, (long long)every);
-    if (nrows < 1) return set_error(YB_EINVAL, "%s: nrows = %lld is less than 1", WHAT, (long long)nrows);
-    // the frames of the whole box, which bound every rank's share, must be addressable (byte counts and row offsets)
-    int64_t points = 1, bytes = 0;
+    if (every < 1) return set_error(YB_EINVAL, "%s: every = %lld is less than 1", what, (long long)every);
+    if (nrows < 1) return set_error(YB_EINVAL, "%s: nrows = %lld is less than 1", what, (long long)nrows);
+    int64_t points = 1;
     bool over = false;
     for (int k = 0; k < s->ndd; k++) over = over || __builtin_mul_overflow(points, r.count[k], &points);
     over = over || __builtin_mul_overflow(points, nrows, &bytes) || __builtin_mul_overflow(bytes, int64_t(s->spec.elem_bytes), &bytes);
     if (over)
         return set_error(YB_ERANGE, "%s: %lld rows of the decimated box (%lld x %lld x %lld points) of %d-byte elements overflow a 64-bit "
-                         "byte count", WHAT, (long long)nrows, (long long)r.count[0], (long long)r.count[1], (long long)r.count[2],
+                         "byte count", what, (long long)nrows, (long long)r.count[0], (long long)r.count[1], (long long)r.count[2],
                          s->spec.elem_bytes);
     r.t0 = t0; r.every = every; r.nrows = nrows;
+    return 0;
+}
+
+// Append r to *pp (created on first use): planned now when the rank geometry is known; on a prepared solution its frames are
+// allocated and the table uploaded now too -- never by run_solution() -- after the work that may read the old table.
+static int install(Solution* s, SlicesState*& pp, bool inject, SliceRec&& r, int64_t* id) {
+    if (!pp) pp = new_state(inject);
+    SlicesState& p = *pp;
     if (geometry_known(*s)) {
-        if (int rc = check_mode(*s)) return rc;
-        if (int rc = plan_one(*s, r)) return rc;
+        if (int rc = check_mode(*s, p)) return rc;
+        if (int rc = plan_one(*s, p, r)) return rc;
     }
-    if (!s->slices) s->slices = new SlicesState();
-    SlicesState& p = *s->slices;
     if (s->prepared) {
-        // frames are allocated here or at prepare, never by run_solution(); the table in use may still be read by queued work
         YB_CUDA(cudaSetDevice(s->device));
         YB_CUDA(cudaStreamSynchronize(s->stream()));
-        if (int rc = alloc_frames(*s, r)) return rc;
-        p.recs.push_back(r);
-        if (int rc = upload_table(*s)) {
+        if (int rc = alloc_frames(*s, p, r)) return rc;
+        p.recs.push_back(std::move(r));
+        if (int rc = upload_table(*s, p)) {
             release(p.recs.back());
             p.recs.pop_back();
             return rc;
         }
     } else {
-        p.recs.push_back(r);
+        p.recs.push_back(std::move(r));
     }
+    if (inject) plan_groups(p);
     if (id) *id = int64_t(p.recs.size()) - 1;
     return 0;
+}
+
+static int clear_state(Solution* s, SlicesState*& p, bool inject) {
+    if (!p) return 0;
+    if (s->prepared) {
+        YB_CUDA(cudaSetDevice(s->device));
+        YB_CUDA(cudaStreamSynchronize(s->stream()));
+    }
+    const int64_t launches = p->launches;
+    slices_free(p);
+    p = new_state(inject);
+    p->launches = launches;
+    return 0;
+}
+
+extern "C" {
+
+int yb_solution_add_slice(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                          int64_t t0, int64_t every, int64_t nrows, int64_t* id) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    SliceRec r;
+    int64_t bytes = 0;
+    if (int rc = new_rec(s, "slice", var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    return install(s, s->slices, false, std::move(r), id);
+}
+
+int yb_solution_add_slice_injector(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                   int64_t t0, int64_t every, int64_t nrows, int mode, const void* frames, int64_t* id) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    const char* what = "slice injector";
+    SliceRec r;
+    int64_t bytes = 0;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (mode != YB_INJECT_ADD && mode != YB_INJECT_SET)
+        return set_error(YB_EINVAL, "%s: unknown mode %d (YB_INJECT_ADD = %d or YB_INJECT_SET = %d)", what, mode, YB_INJECT_ADD, YB_INJECT_SET);
+    if (!frames) return set_error(YB_EINVAL, "%s: null frames", what);
+    r.mode = mode;
+    try {
+        r.host_frames.assign(static_cast<const char*>(frames), static_cast<const char*>(frames) + bytes);
+    } catch (const std::exception&) {
+        return set_error(YB_ENOMEM, "%s: cannot copy %lld bytes of frames on the host", what, (long long)bytes);
+    }
+    return install(s, s->injectors, true, std::move(r), id);
 }
 
 int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t* owned) {
@@ -285,16 +532,12 @@ int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t
     if (!geometry_known(*s)) return set_error(YB_ESTATE, "get_slice_frames: the rank geometry is not known yet (plan_geometry / prepare_solution)");
     SliceRec& r = s->slices->recs[size_t(id)];
     if (!s->prepared)
-        if (int rc = plan_one(*s, r)) return rc;
-    const int nd = s->ndd;
-    int64_t cnt[3] = {1, 1, 1}, k0[3] = {0, 0, 0}, kn[3] = {1, 1, 1};
-    for (int k = 0; k < nd; k++) { cnt[k] = r.count[k]; k0[k] = r.own_k0[k]; kn[k] = r.own_n[k]; }
-    const size_t box = size_t(cnt[0] * cnt[1] * cnt[2]);
+        if (int rc = plan_one(*s, *s->slices, r)) return rc;
+    size_t box = 1;
+    for (int k = 0; k < s->ndd; k++) box *= size_t(r.count[k]);
     if (owned) {
         memset(owned, 0, box);
-        for (int64_t a = 0; a < kn[0]; a++)
-            for (int64_t b = 0; b < kn[1]; b++)
-                memset(owned + ((k0[0] + a) * cnt[1] + k0[1] + b) * cnt[2] + k0[2], 1, size_t(kn[2]));
+        owned_runs(*s, r, 1, [&](size_t whole, size_t, size_t n) { memset(owned + whole, 1, n); });
     }
     if (!out) return 0;
     const size_t eb = size_t(s->spec.elem_bytes);
@@ -304,28 +547,20 @@ int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t
     YB_CUDA(cudaSetDevice(s->device));
     YB_CUDA(cudaMemcpyAsync(dense.data(), r.d_frames, dense.size(), cudaMemcpyDeviceToHost, s->stream()));
     YB_CUDA(cudaStreamSynchronize(s->stream()));
-    const char* src = dense.data();
-    for (int64_t row = 0; row < r.nrows; row++)
-        for (int64_t a = 0; a < kn[0]; a++)
-            for (int64_t b = 0; b < kn[1]; b++, src += size_t(kn[2]) * eb)
-                memcpy(static_cast<char*>(out) + ((size_t(row) * cnt[0] + k0[0] + a) * cnt[1] + k0[1] + b) * cnt[2] * eb + size_t(k0[2]) * eb, src,
-                       size_t(kn[2]) * eb);
+    owned_runs(*s, r, r.nrows, [&](size_t whole, size_t own, size_t n) { memcpy(static_cast<char*>(out) + whole * eb, dense.data() + own * eb, n * eb); });
     return 0;
 }
 
 int yb_solution_clear_slices(yb_solution* s_) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
-    if (!s->slices) return 0;
-    if (s->prepared) {
-        YB_CUDA(cudaSetDevice(s->device));
-        YB_CUDA(cudaStreamSynchronize(s->stream()));
-    }
-    const int64_t launches = s->slices->launches;
-    slices_free(s->slices);
-    s->slices = new SlicesState();
-    s->slices->launches = launches;
-    return 0;
+    return clear_state(s, s->slices, false);
+}
+
+int yb_solution_clear_slice_injectors(yb_solution* s_) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    return clear_state(s, s->injectors, true);
 }
 
 }  // extern "C"

@@ -1,10 +1,16 @@
-// Slice recorders: boxes of a var recorded on the device inside run_solution() (yb_slices.cu).
+// Slice recorders and slice injectors: boxes of a var recorded from, or written into, the device inside run_solution()
+// (yb_slices.cu).
 //
 // A recorder names a var, an inclusive box [first, last] of global domain indices with a stride per dim, and a step window:
 // step u (the step a run has just computed) is recorded into frame row (u - t0) / every when u - t0 is a multiple of `every` and
 // that row is below nrows.  A frame row holds what get_elements_in_slice of the decimated box would read right after the
 // run_solution() call that computed u -- after that step's sources and receivers (yb_points.h).  Each rank records and stores
 // only its own part of the decimated box.
+//
+// An injector is the dual: the same box and window, and frames given by the caller.  When row r is due at step u it sets
+// (YB_INJECT_SET) or adds to (YB_INJECT_ADD, one add in the element type) var(u) at every point of the decimated box, right after
+// the step's stages and before its sources, receivers and recorders.  Injectors run in id order: the list is split into launch
+// groups, a new group starting where an injector's box meets an earlier member's on the same var.
 #pragma once
 #include "yb_core.h"
 
@@ -24,27 +30,41 @@ struct SliceRec {
     // the var's storage and slot_bias as the device table holds them (fuse_vars and the offline tuner's pairs move them)
     const void* uploaded_base = nullptr;
     int uploaded_bias = -1;
+    // injectors only
+    int mode = 0;                               // YB_INJECT_ADD / YB_INJECT_SET
+    std::vector<char> host_frames;              // the caller's frames (nrows x the whole decimated box) until uploaded
 };
 
 struct SlicesState {
+    const char* what = "slice";                 // message prefix: "slice" (recorders) or "slice injector"
+    bool inject = false;
     std::vector<SliceRec> recs;
     void* d_table = nullptr;                    // one descriptor per recorder (yb_slices.cu)
     size_t table_cap = 0;                       // descriptors d_table has room for
     int num_sms = 0;                            // of the solution's device, read with the table
-    int64_t launches = 0;                       // recording launches since prepare (read-only option slice_launches)
+    int64_t launches = 0;                       // launches since prepare (read-only options slice_launches, slice_injector_launches)
+    std::vector<int> group_first;               // injectors: launch group g is recs[group_first[g] .. group_first[g + 1])
 };
 
 void slices_free(SlicesState* p);
-void slices_preload();                          // load the recording kernel now (preload_kernel)
+void slices_preload();                          // load the recording and injecting kernels now (preload_kernel)
 bool slices_active(const Solution& s);
-// validation + this rank's part of every recorder (host only: needs the rank geometry, no device)
+bool slice_injectors_active(const Solution& s);
+// validation + this rank's part of every recorder and injector (host only: needs the rank geometry, no device)
 int slices_plan(Solution& s);
-// plan, then allocate the frames of every recorder and upload the descriptor table (prepare_solution)
+// plan, then allocate the frames of every recorder and injector and upload the descriptor tables (prepare_solution)
 int slices_prepare(Solution& s);
-// before a run enqueues anything: refresh the descriptor table if a var's storage (fuse_vars) or live slots (a temporal tile
-// of the offline tuner) moved since it was uploaded; never allocates a frame buffer
+// before a run enqueues anything: refresh the descriptor tables if a var's storage (fuse_vars) or live slots (a temporal tile
+// of the offline tuner) moved since they were uploaded; never allocates a frame buffer
 int slices_begin_run(Solution& s);
 // the recording launch of step t (the step the stage loop just computed from t): returns #kernels launched (0 or 1) or <0
 int slices_launch(Solution& s, int64_t t, cudaStream_t st);
+// the injecting launches of step t, one per launch group with a row due, in id order; sel (PTS_*) picks the points outside or
+// inside `interior` (rank-local) on a rank grid's split form.  Returns #kernels launched or <0
+int slice_injectors_launch(Solution& s, int64_t t, int sel, const Box& interior, cudaStream_t st);
+// rank-local x range [x0, x1] of the points this rank injects at step t; false when it injects none
+bool slice_injectors_x_range(const Solution& s, int64_t t, int64_t& x0, int64_t& x1);
+// read-only option slice_injector_groups: the launch groups in order separated by ';', each its comma-separated ids ("0,1;2")
+std::string slice_injector_groups_text(const Solution& s);
 
 }  // namespace yb

@@ -990,4 +990,36 @@ idx_t yk_get_slice_launches(yk_solution_ptr soln) {
     return idx_t(atoll(v));
 }
 
+idx_t yk_add_slice_injector(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                            idx_t nrows, const std::vector<double>& frames, const idx_t_vec& stride, idx_t every, bool set) {
+    B200Solution& s = b200_slices(soln);
+    const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
+    if (first.size() != nd || last.size() != nd || (!stride.empty() && stride.size() != nd))
+        fail("slice injector: first, last and stride need " + std::to_string(nd) + " domain indices each");
+    const std::vector<int64_t> f(first.begin(), first.end()), l(last.begin(), last.end()), st(stride.begin(), stride.end());
+    size_t n = nrows > 0 ? size_t(nrows) : 0;
+    for (size_t k = 0; k < nd; k++) n *= l[k] >= f[k] && (st.empty() || st[k] > 0) ? size_t((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1) : 0;
+    if (n && frames.size() != n)
+        fail("slice injector: " + std::to_string(frames.size()) + " frame values given, nrows x the decimated box is " + std::to_string(n));
+    int64_t id = -1;
+    const int mode = set ? YB_INJECT_SET : YB_INJECT_ADD;
+    if (yb_solution_elem_bytes(s.h->s) == 4) {
+        const std::vector<float> fr(frames.begin(), frames.end());       // rounded once to the element type
+        chk(yb_solution_add_slice_injector(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, mode,
+                                           fr.data(), &id));
+    } else {
+        chk(yb_solution_add_slice_injector(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, mode,
+                                           frames.data(), &id));
+    }
+    return idx_t(id);
+}
+
+void yk_clear_slice_injectors(yk_solution_ptr soln) { chk(yb_solution_clear_slice_injectors(b200_slices(soln).h->s)); }
+
+idx_t yk_get_slice_injector_launches(yk_solution_ptr soln) {
+    char v[64];
+    chk(yb_get_option(b200_slices(soln).h->s, "slice_injector_launches", v, sizeof v));
+    return idx_t(atoll(v));
+}
+
 }  // namespace yask

@@ -317,4 +317,9 @@ PYBIND11_MODULE(yask_kernel, m) {
     }, py::arg("soln"), py::arg("id"), "(frames as a flat list of floats, shape (nrows, box extents...), owned per box point)");
     m.def("yk_clear_slices", &yk_clear_slices, py::arg("soln"));
     m.def("yk_get_slice_launches", &yk_get_slice_launches, py::arg("soln"));
+    // ---- slice injectors on the device (yask_b200_slices.hpp; not in the reference API) ----
+    m.def("yk_add_slice_injector", &yk_add_slice_injector, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"), py::arg("t0"),
+          py::arg("nrows"), py::arg("frames"), py::arg("stride") = idx_t_vec{}, py::arg("every") = 1, py::arg("set") = false);
+    m.def("yk_clear_slice_injectors", &yk_clear_slice_injectors, py::arg("soln"));
+    m.def("yk_get_slice_injector_launches", &yk_get_slice_injector_launches, py::arg("soln"));
 }

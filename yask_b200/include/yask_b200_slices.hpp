@@ -1,4 +1,4 @@
-// Slice recorders on the device inside run_solution(): an extension of the C++ kernel API of this engine.
+// Slice recorders and injectors on the device inside run_solution(): an extension of the C++ kernel API of this engine.
 //
 // The reference API has no such calls; its users record a receiver plane or a snapshot from the host, one step at a time:
 //
@@ -28,5 +28,21 @@ void yk_get_slice_frames(yk_solution_ptr soln, idx_t id, std::vector<double>& fr
 void yk_clear_slices(yk_solution_ptr soln);
 // Recording launches since prepare_solution().
 idx_t yk_get_slice_launches(yk_solution_ptr soln);
+
+// Slice injectors, the dual of the recorders: replaces the host loop
+//
+//     soln->run_solution(t);  p->get_elements_in_slice(box, ...);  box[::stride] (+)= frame[r];  p->set_elements_in_slice(box, ...);
+//
+// After every step u a run computes, if u - t0 is a multiple of `every` and r = (u - t0) / every < nrows, frame r is set into
+// (set = true) or added to (one add in the element type) var(u) at first[d], first[d] + stride[d], ... <= last[d], before that
+// step's sources, receivers and recorders.  frames: nrows x the decimated box, row-major, the last domain dim fastest, given as
+// doubles and rounded once to the element type.  Semantics and the rank-grid rules: yb_solution_add_slice_injector in
+// include/yask_b200.h.  Returns the injector's id (0, 1, ... until yk_clear_slice_injectors; separate from the recorders').
+idx_t yk_add_slice_injector(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                            idx_t nrows, const std::vector<double>& frames, const idx_t_vec& stride = {}, idx_t every = 1, bool set = false);
+// Remove every injector: later runs take their usual launch path again.
+void yk_clear_slice_injectors(yk_solution_ptr soln);
+// Injecting launches since prepare_solution().
+idx_t yk_get_slice_injector_launches(yk_solution_ptr soln);
 
 }  // namespace yask
