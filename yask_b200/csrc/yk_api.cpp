@@ -9,6 +9,7 @@
 #include "../include/yask_b200_slices.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
@@ -391,14 +392,25 @@ struct B200Var : yk_var {
         chk(yb_var_set_slice_same(h->s, vi, val, ff.data(), ll.data(), &done));
         return done;
     }
-    yk_reduction_result_ptr reduce_elements_in_slice(int mask, const idx_t_vec& f, const idx_t_vec& l, bool) override {
+    yk_reduction_result_ptr reduce_elements_in_slice(int mask, const idx_t_vec& f, const idx_t_vec& l, bool strict) override {
         need_storage("reduce_elements_in_slice");
-        (void)slice_elems(f, l);   // validates the index vectors
+        auto i = info();
+        if (int(f.size()) != i.num_dims || int(l.size()) != i.num_dims) fail("reduce_elements_in_slice: wrong number of indices for var '" + name + "'");
         auto r = std::make_shared<B200Reduction>();
+        r->mask = mask; r->mx = -HUGE_VAL; r->mn = HUGE_VAL;
+        idx_t_vec ff(f), ll(l);
+        if (!strict) {   // clip every index to the local range (check_indices, yk_var.cpp:485-545); nothing left: num 0, initial values
+            for (int k = 0; k < i.num_dims; k++) {
+                if (i.dims[k].kind == 0 && *step_wrap) continue;
+                ff[k] = std::max(ff[k], first_local(i, k));
+                ll[k] = std::min(ll[k], last_local(i, k));
+                if (ll[k] < ff[k]) return r;
+            }
+        }
         double out[5];
         int64_t n = 0;
-        chk(yb_var_reduce_slice(h->s, vi, f.data(), l.data(), out, &n));   // on the device, in double
-        r->mask = mask; r->n = idx_t(n);
+        chk(yb_var_reduce_slice(h->s, vi, ff.data(), ll.data(), out, &n));   // on the device, in double
+        r->n = idx_t(n);
         r->sum = out[0]; r->sumsq = out[1]; r->prod = out[2]; r->mx = out[3]; r->mn = out[4];
         return r;
     }
