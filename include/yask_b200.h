@@ -306,6 +306,40 @@ enum { YB_INJECT_ADD = 0, YB_INJECT_SET = 1 };
 int yb_solution_add_slice_injector(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
                                    int64_t t0, int64_t every, int64_t nrows, int mode, const void* frames, int64_t* id);
 int yb_solution_clear_slice_injectors(yb_solution* s);   /* remove every injector and free its frames; ids restart at 0 */
+/* An injector as yb_solution_add_slice_injector whose frames are those of recorder `src_id` of solution `src` (which may be `s`),
+ * read on the device with no copy: row r reads recorder row reverse ? nrows - 1 - r : r, with this injector's nrows.  The
+ * frames are shared as described at yb_solution_add_slice_correlator, with the same checks and the same ordering. */
+int yb_solution_add_slice_injector_from(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                        int64_t t0, int64_t every, int64_t nrows, int mode, yb_solution* src, int64_t src_id, int reverse,
+                                        int64_t* id);
+
+/* ---- slice correlators: the imaging condition accumulated on the device inside run_solution() ----------------------------
+ * For the adjoint run of a reverse-time shot: image(x) += S(x, u) * R(x, u) summed over the correlated steps, where S is the
+ * forward wavefield kept as a recorder's frames and R the var.  It replaces the host loop run_solution(t, t);
+ * get_elements_in_slice(box, {u, first...}, {u, last...}); image += frame[row] * box[::stride] with one call, bit for bit.  The
+ * box (first, last, stride), the window (t0, every, nrows) and the var rules are those of yb_solution_add_slice.  The image is one
+ * frame of the decimated box in the element type T, zeroed when it is allocated; each rank holds its own part.  Whenever a run
+ * has computed step u, if u - t0 is a multiple of `every` and r = (u - t0) / every is in [0, nrows), then for every point pt:
+ *   image[pt] = T(image[pt] + T(var(u, pt) * b[pt])), the product and the sum each rounded (no FMA),
+ * where b = var(u) when `src` is NULL (autocorrelation: the source illumination), otherwise row reverse ? nrows - 1 - r : r of
+ * recorder `src_id` of solution `src` (which may be `s`), as that row stands when the launch runs in stream order.  Within step
+ * u: injectors, sources, receivers, recorders, then the correlators, all due ones in one launch.  Images accumulate across runs.
+ * Frames shared from a recorder: the consumer holds a reference, so clear_slices on `src` or destroying `src` leaves it reading
+ * the frames as they were.  Refused unless `src` has recorder src_id with this box and stride and at least nrows rows, the same
+ * element bytes and domain dims, and (both with their rank geometry) the same overall domain, rank grid and rank index; then
+ * unless `src` is prepared, so the frames exist; `reverse` is 0 or 1; a consumer planned before its prepare is checked again then,
+ * with the device.  Between two solutions runs behave as if executed in the order the host enqueued them: a consumer's run waits
+ * for the source's last run, and a source's run for the last runs of its consumers.  Images are allocated at this call on a
+ * prepared solution (which synchronizes its stream), otherwise at prepare -- never in run_solution().  While any correlator is
+ * set every run takes one step per launch; a fused-pair rank grid refuses them.  *id (0, 1, ...) names the correlator; ids are
+ * separate from the recorders' and injectors'.  Read-only option slice_correlator_launches: correlating launches since prepare
+ * (one per step in which some correlator of this rank has a row due). */
+int yb_solution_add_slice_correlator(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                     int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id);
+/* The image of correlator `id` as the whole decimated box in the solution's type (0 where this rank owns no point) and the owned
+ * mask, as yb_solution_get_slice_frames with one row. */
+int yb_solution_get_correlator_image(yb_solution* s, int64_t id, void* out, uint8_t* owned);
+int yb_solution_clear_slice_correlators(yb_solution* s);   /* remove every correlator and free its image; ids restart at 0 */
 
 /* ---- multi-GPU halo exchange, one process per GPU (replaces exchange_halos, halo.cpp:80-491) --- */
 /* Each rank exports an opaque blob (CUDA IPC handles of its var storage + sync flags), the

@@ -63,7 +63,8 @@ ABI_SYMBOLS = [
     "yb_get_stats", "yb_clear_stats", "yb_solution_set_sources", "yb_solution_set_receivers", "yb_solution_get_traces",
     "yb_solution_clear_points", "yb_solution_set_sources_weighted", "yb_solution_set_receivers_weighted", "yb_points_trilinear",
     "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
-    "yb_solution_add_slice_injector", "yb_solution_clear_slice_injectors",
+    "yb_solution_add_slice_injector", "yb_solution_clear_slice_injectors", "yb_solution_add_slice_injector_from",
+    "yb_solution_add_slice_correlator", "yb_solution_get_correlator_image", "yb_solution_clear_slice_correlators",
     "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
@@ -143,6 +144,12 @@ def lib() -> C.CDLL:
         L.yb_solution_add_slice_injector.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, i32, p,
                                                      C.POINTER(i64)]
         L.yb_solution_clear_slice_injectors.argtypes = [p]
+        L.yb_solution_add_slice_injector_from.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, i32,
+                                                          p, i64, i32, C.POINTER(i64)]
+        L.yb_solution_add_slice_correlator.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, p, i64,
+                                                       i32, C.POINTER(i64)]
+        L.yb_solution_get_correlator_image.argtypes = [p, i64, p, C.POINTER(C.c_uint8)]
+        L.yb_solution_clear_slice_correlators.argtypes = [p]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
         L.yb_halo_export.argtypes = [p, p, C.c_size_t]
         L.yb_halo_import.argtypes = [p, i64, p, C.c_size_t]
@@ -577,6 +584,63 @@ class Solution:
 
     def clear_slice_injectors(self):
         _chk(lib().yb_solution_clear_slice_injectors(self._h))
+
+    def _box(self, what, first, last, stride):
+        nd = len(self.get_domain_dim_names())
+        f, l = np.atleast_1d(np.asarray(first, np.int64)), np.atleast_1d(np.asarray(last, np.int64))
+        st = np.ones(nd, np.int64) if stride is None else np.atleast_1d(np.asarray(stride, np.int64))
+        for name, a in (("first", f), ("last", l), ("stride", st)):
+            if a.shape != (nd,):
+                raise YaskError(-1, f"{what}: {name} needs {nd} domain index(es) ({', '.join(self.get_domain_dim_names())}), "
+                                    f"got {a.tolist()}")
+        return f, l, st
+
+    def add_slice_injector_from(self, var: str, first, last, t0: int, nrows: int, src: "Solution", src_id: int, reverse: bool = False,
+                                stride=None, every: int = 1, mode: str = "add") -> int:
+        """add_slice_injector with the frames of recorder src_id of solution src (which may be this one), read on the device with
+        no copy: row r reads recorder row nrows - 1 - r when reverse, else r.  Returns the injector's id."""
+        f, l, st = self._box("slice injector", first, last, stride)
+        if mode not in self.INJECT_MODES:
+            raise YaskError(-1, f"slice injector: unknown mode {mode!r} (expected 'add' or 'set')")
+        rid = C.c_int64(-1)
+        _chk(lib().yb_solution_add_slice_injector_from(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                       int(t0), int(every), int(nrows), self.INJECT_MODES[mode], src._h, int(src_id),
+                                                       int(reverse), C.byref(rid)))
+        return rid.value
+
+    # slice correlators (yb_solution_add_slice_correlator / get_correlator_image / clear_slice_correlators)
+    def add_slice_correlator(self, var: str, first, last, t0: int, nrows: int, src: "Solution" = None, src_id: int = None,
+                             reverse: bool = False, stride=None, every: int = 1) -> int:
+        """After every step u a run computes with u - t0 a multiple of `every` and r = (u - t0) // every below nrows, add
+        var(u) * b to the image at the box first[d], first[d] + stride[d], ... <= last[d], the product and the sum each rounded to
+        the element type.  b is var(u) with no src (the illumination), else row r (nrows - 1 - r when reverse) of recorder src_id
+        of solution src (which may be this one).  Returns the correlator's id."""
+        f, l, st = self._box("slice correlator", first, last, stride)
+        if src is not None and src_id is None:
+            raise YaskError(-1, "slice correlator: a source solution needs src_id, the id of one of its recorders")
+        rid = C.c_int64(-1)
+        _chk(lib().yb_solution_add_slice_correlator(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                    int(t0), int(every), int(nrows), None if src is None else src._h,
+                                                    0 if src_id is None else int(src_id), int(reverse), C.byref(rid)))
+        if not hasattr(self, "_correlators"):
+            self._correlators = {}
+        self._correlators[rid.value] = tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1)
+        return rid.value
+
+    def get_correlator_image(self, cid: int):
+        """(image, owned): image (box_shape) in the element dtype, owned (box_shape) True for the points this rank holds; the
+        others stay 0."""
+        shape = getattr(self, "_correlators", {}).get(cid, (0,))
+        dt = np.float32 if self.get_element_bytes() == 4 else np.float64
+        out = np.zeros(shape, dtype=dt)
+        owned = np.zeros(shape, dtype=np.uint8)
+        _chk(lib().yb_solution_get_correlator_image(self._h, int(cid), out.ctypes.data if self.is_prepared() else None,
+                                                    owned.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return out, owned.astype(bool)
+
+    def clear_slice_correlators(self):
+        _chk(lib().yb_solution_clear_slice_correlators(self._h))
+        self._correlators = {}
 
     def is_prepared(self) -> bool:
         return bool(lib().yb_solution_is_prepared(self._h))

@@ -44,6 +44,7 @@ Solution::~Solution() {
     points_free(points);     // device tables are released on `device`, selected above
     slices_free(slices);
     slices_free(injectors);
+    slices_free(correlators);
 }
 
 static int check_dim(const Solution* s, int dim) {
@@ -407,7 +408,7 @@ int yb_set_option(yb_solution* s_, const char* key, const char* value) {
         s->tuner = Solution::InRunTuner();
         s->tuner.enabled = atoi(value) != 0;
     } else if (k == "point_launches" || k == "point_groups" || k == "slice_launches" || k == "slice_injector_groups" ||
-               k == "slice_injector_launches") {
+               k == "slice_injector_launches" || k == "slice_correlator_launches") {
         return set_error(YB_EINVAL, "option '%s' is read-only", key);
     } else if (k == "overlap_comms" || k == "min_exterior" || k == "fused_halo" || k == "dma_halo") {
         // consumed by the halo engine at run time
@@ -427,6 +428,7 @@ int yb_get_option(const yb_solution* s_, const char* key, char* value, size_t n)
     else if (std::string(key) == "slice_launches") v = std::to_string(s->slices ? s->slices->launches : 0);   // read-only
     else if (std::string(key) == "slice_injector_groups") v = slice_injector_groups_text(*s);                   // read-only
     else if (std::string(key) == "slice_injector_launches") v = std::to_string(s->injectors ? s->injectors->launches : 0);   // read-only
+    else if (std::string(key) == "slice_correlator_launches") v = std::to_string(s->correlators ? s->correlators->launches : 0);   // read-only
     else if (!s->engine->get_option(*s, key, v)) {
         auto it = s->options.find(key);
         if (it == s->options.end()) return set_error(YB_EINVAL, "unknown option '%s'", key);
@@ -462,7 +464,7 @@ int yb_solution_plan_geometry(yb_solution* s_) {
     if (int rc = s->engine->check_geometry(*s)) return rc;
     if (points_active(*s))
         if (int rc = points_plan(*s)) return rc;          // point sets given before the geometry are checked now
-    return slices_plan(*s);                               // and so are slice recorders and injectors
+    return slices_plan(*s);                               // and so are slice recorders, injectors and correlators
 }
 
 int yb_solution_prepare(yb_solution* s_, int device) {
@@ -506,9 +508,10 @@ int yb_solution_prepare(yb_solution* s_, int device) {
     if (s->multi_rank()) {
         if (int rc = halo_prepare(*s)) return rc;
     }
-    if (int rc = slices_prepare(*s)) return rc;       // frames of the recorders and injectors added before prepare
+    if (int rc = slices_prepare(*s)) return rc;       // frames and images of the slices added before prepare
     if (s->slices) s->slices->launches = 0;
     if (s->injectors) s->injectors->launches = 0;
+    if (s->correlators) s->correlators->launches = 0;
     YB_CUDA(cudaStreamSynchronize(s->stream()));
     s->prepared = true;
     memset(&s->stats, 0, sizeof s->stats);
@@ -848,6 +851,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     // point tables are normally uploaded when they are set (or at prepare); before anything of this run is enqueued otherwise
     if (int rc = points_begin_run(*s)) return rc;
     if (int rc = slices_begin_run(*s)) return rc;
+    if (int rc = slices_run_waits(*s, st)) return rc;     // frames shared with other solutions (yb_slices.h)
     // Timing events: pairs of finished runs are folded into the stats and recycled here, so that calling
     // run_solution(t) once per step (the reference's usual pattern) keeps a bounded number of events alive.
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -882,10 +886,11 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     // Temporal tile (the reference's "-bt", context.cpp:657-681): a forward run goes through the engine's fused launch, `fs` steps
     // at a time; what is left over (and every other kind of run) takes the one-step path below.  A rank grid fuses steps only
     // in the mode its engine fixed at prepare; its halos are then 2R deep and exchanged once per fused launch.  Point sources
-    // and slice injectors enter between two steps, and slice recorders read a step a pair would never store, so a solution with
-    // any of them runs one step per launch (all are refused on a rank grid in the fused mode).
+    // and slice injectors enter between two steps, and slice recorders and correlators read a step a pair would never store, so a
+    // solution with any of them runs one step per launch (all are refused on a rank grid in the fused mode).
     int64_t t_first = first_step;
-    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s) && !slices_active(*s) && !slice_injectors_active(*s))
+    const int fs = (step_dir > 0 && (s->halo || !s->tuner.enabled) && !points_active(*s) && !slices_active(*s) && !slice_injectors_active(*s) &&
+                    !slice_correlators_active(*s))
                        ? s->engine->fused_steps(*s) : 1;
     if (s->halo && fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) rc = halo_exchange_deep(*s, t_first, true, st);
     while (fs > 1 && rc >= 0 && last_step - t_first + 1 >= fs) {
@@ -938,6 +943,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
         if (rc >= 0 && !s->halo) rc = points_launch(*s, t, PTS_ALL, whole, st);
         // then the slice recorders, before the next step's first launch can overwrite an in-place var (halo_run_stage on a grid)
         if (rc >= 0 && !s->halo) rc = slices_launch(*s, t, st);
+        if (rc >= 0 && !s->halo) rc = slice_correlators_launch(*s, t, st);    // which see that step's recording
         s->stats.num_steps_done++;
         if (tv >= 0 && te0 && te1) {
             cudaEventRecord(te1, st);
@@ -964,6 +970,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     }
     if (s->halo && rc >= 0) rc = halo_finish(*s, st);   // the last exchange completes inside the run (and its timing)
     if (s->halo && rc >= 0) rc = points_record_pending(*s, st);        // then the last step's weighted receivers
+    if (int e = slices_run_records(*s, st)) return e;
     YB_CUDA(cudaEventRecord(e1, st));
     return rc < 0 ? rc : 0;
 }

@@ -223,6 +223,8 @@ struct Solution {
     SlicesState* slices = nullptr;   // owned; freed by slices_free()
     // slice injectors (yb_slices.h)
     SlicesState* injectors = nullptr;   // owned; freed by slices_free()
+    // slice correlators (yb_slices.h)
+    SlicesState* correlators = nullptr;   // owned; freed by slices_free()
     // Fused halo stores (set by the halo layer before a stage launch, consumed by an engine that can store its
     // boundary planes straight into the x neighbours' halo cells): element (0,0,0)-relative base pointers of the
     // OUTPUT var's step slot in the lower / upper x neighbour, or null.  The engine sets `used` if it honoured them.

@@ -504,7 +504,8 @@ static bool other_dirty(const HaloState* h, int var, int slot) {
 // pushes and the rest after the interior launch, so every point is written once and before the exchange that publishes it.
 // Slice recorders (yb_slices.h) only read: they record in the last stage, after the launch that computed the rank's last points
 // and that launch's points (fused: the launch; whole: the launch; split: the interior launch), on this stream, so before the next
-// step's first launch overwrites an in-place var.  They never change the form.
+// step's first launch overwrites an in-place var.  They never change the form.  Slice correlators only read the var too: they
+// follow the recorders in the same places.
 // Does this rank write at step t, after the last stage's launch, within w planes of an x interface with a neighbour rank (point
 // sources, slice injectors)?  Such a write must come before the boundary planes are published, which the fused x launch does itself.
 static bool writes_near_x_interface(const Solution& s, int64_t t, int64_t w) {
@@ -536,7 +537,13 @@ int halo_run_stage(Solution& s, int stage, int64_t t, cudaStream_t st) {
         const int b = points_launch(s, t, sel, interior, st);
         return b < 0 ? b : a + b;
     };
-    auto record_slices = [&]() { return last_stage ? slices_launch(s, t, st) : 0; };
+    auto record_slices = [&]() {
+        if (!last_stage) return 0;
+        const int a = slices_launch(s, t, st);
+        if (a < 0) return a;
+        const int b = slice_correlators_launch(s, t, st);
+        return b < 0 ? b : a + b;
+    };
     int64_t wx = 0;         // widest x halo: the planes of an x interface the neighbour reads
     for (auto& v : s.vars)
         if (const Dim* dx = v.domain_dim(0)) wx = std::max({wx, dx->spec.halo_l, dx->spec.halo_r});

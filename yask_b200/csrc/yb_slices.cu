@@ -2,7 +2,9 @@
 // inside run_solution() by one many-CTA launch per step, instead of the reference API loop run_solution(t, t) /
 // get_elements_in_slice, which pays a synchronous device-to-host copy per frame and loses the temporal tile's pairs.  Slice
 // injectors write boxes back the same way (plane-wave and areal sources, boundary replay, time-varying Dirichlet data), instead of
-// the loop run_solution(t, t) / get_elements_in_slice / set_elements_in_slice.
+// the loop run_solution(t, t) / get_elements_in_slice / set_elements_in_slice.  Slice correlators accumulate the imaging condition
+// image += var(u) * frame into an image on the device, the frames being var(u) itself or a recorder's, instead of the loop
+// run_solution(t, t) / get_elements_in_slice / host arithmetic.
 #include <stdio.h>
 #include <string.h>
 
@@ -26,7 +28,10 @@ struct SliceDesc {
     int alloc, bias, step_off;      // Var::slot_of(u) = imod(u, alloc) + bias
     long long t0, every, nrows;
     BoxDev box;                     // this rank's part: element offset of its first point, decimated strides
-    char* frames;                   // nrows x box.total elements
+    char* frames;                   // nrows x box.total elements (correlators: null for an autocorrelation)
+    char* image;                    // correlators: box.total elements
+    int rev;                        // row r reads frame row nrows - 1 - r
+    int lanes_log2;                 // correlators: threads per row of the unit-stride dim, a power of two up to 256
     // injectors: YB_INJECT_ADD / SET, and the rank-local coordinates of the first owned point and their step per box index
     // (dims right-aligned as in box), which the split form's selection tests against the interior box
     int mode;
@@ -83,7 +88,7 @@ __global__ void __launch_bounds__(256) slice_injectors_kernel(const SliceDesc* _
         long long slot = u % d.alloc;
         slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
         T* __restrict__ dst = reinterpret_cast<T*>(const_cast<char*>(d.var_base) + slot * d.slot_bytes);
-        const T* __restrict__ src = reinterpret_cast<const T*>(d.frames) + row * b.total;
+        const T* __restrict__ src = reinterpret_cast<const T*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total;
         const bool set = d.mode == YB_INJECT_SET;
         long long coord[4];
         for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) {
@@ -102,31 +107,129 @@ __global__ void __launch_bounds__(256) slice_injectors_kernel(const SliceDesc* _
     }
 }
 
+// the imaging condition's rounding: the product and the sum each rounded, never fused
+__device__ __forceinline__ float mul_add_rn(float img, float v, float b) { return __fadd_rn(img, __fmul_rn(v, b)); }
+__device__ __forceinline__ double mul_add_rn(double img, double v, double b) { return __dadd_rn(img, __dmul_rn(v, b)); }
+
+// blockIdx.y walks the correlators (each writes only its own image, so all the due ones share a launch).  blockIdx.x and the
+// threads walk rows of the unit-stride dim, 2^lanes_log2 threads per row: a row's storage offset is computed once, with the two
+// 64-bit divisions that split the row index, and the lanes step along it, so a full-volume correlator reads var, frame and image
+// contiguously and stays bound by memory, not by per-point index arithmetic.  Offsets are 64-bit: a slot may hold more than 2^31
+// elements.
+template <typename T>
+__global__ void __launch_bounds__(256) slice_correlators_kernel(const SliceDesc* __restrict__ table, int n, long long t) {
+    for (int r = blockIdx.y; r < n; r += gridDim.y) {
+        const SliceDesc& d = table[r];
+        const long long u = t + d.step_off;
+        long long row;
+        if (!row_due(u, d.t0, d.every, d.nrows, row)) continue;
+        const BoxDev b = d.box;
+        long long slot = u % d.alloc;
+        slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
+        const T* __restrict__ var = reinterpret_cast<const T*>(d.var_base + slot * d.slot_bytes) + b.off;
+        const T* __restrict__ src = d.frames ? reinterpret_cast<const T*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total : nullptr;
+        T* __restrict__ img = reinterpret_cast<T*>(d.image);
+        const int lg = d.lanes_log2, lanes = 1 << lg;
+        const long long len = b.n[3], vs = b.vs[3], rows = b.n[0] * b.n[1] * b.n[2], per = 256 >> lg;
+        const int lane = threadIdx.x & (lanes - 1);
+        for (long long q = blockIdx.x * per + (threadIdx.x >> lg); q < rows; q += gridDim.x * per) {
+            const long long q1 = q / b.n[2], c2 = q - q1 * b.n[2];
+            const long long c0 = q1 / b.n[1], c1 = q1 - c0 * b.n[1];
+            const T* __restrict__ vrow = var + c0 * b.vs[0] + c1 * b.vs[1] + c2 * b.vs[2];
+            const long long o = q * len;
+            if (src) {
+                for (long long i = lane; i < len; i += lanes) img[o + i] = mul_add_rn(img[o + i], vrow[i * vs], src[o + i]);
+            } else {
+                for (long long i = lane; i < len; i += lanes) {
+                    const T v = vrow[i * vs];
+                    img[o + i] = mul_add_rn(img[o + i], v, v);
+                }
+            }
+        }
+    }
+}
+
 // The x grid is a grid-stride cap: 8 CTAs per SM is two waves at the 4 CTAs of 256 threads per SM that the kernel's 56
 // registers allow.  y: the hardware limit of gridDim.y; more recorders are walked by the y loop.
 constexpr int CTAS_PER_SM = 8, MAX_GRID_Y = 65535;
 
+// A device buffer freed with cudaFree on its device by its last holder: a recorder's frames outlive the recorder, and its solution,
+// while a consumer holds them.
+std::shared_ptr<void> device_buffer(void* ptr, int device) {
+    return std::shared_ptr<void>(ptr, [device](void* q) {
+        int cur = -1;
+        const bool had = cudaGetDevice(&cur) == cudaSuccess;
+        cudaSetDevice(device);
+        cudaFree(q);
+        if (had) cudaSetDevice(cur);
+    });
+}
+
 void release(SliceRec& r) {
-    if (r.d_frames) cudaFree(r.d_frames);
-    r.d_frames = nullptr;
+    r.frames.reset();
+    r.image.reset();
+    r.link.reset();
     r.uploaded_bias = -1;
     r.uploaded_base = nullptr;
 }
 
-SlicesState* new_state(bool inject) {
+SlicesState* new_state(SliceKind kind) {
     SlicesState* p = new SlicesState();
-    p->inject = inject;
-    p->what = inject ? "slice injector" : "slice";
+    p->kind = kind;
+    p->what = kind == SLICE_INJECT ? "slice injector" : kind == SLICE_CORRELATE ? "slice correlator" : "slice";
     return p;
+}
+
+const char* plural(const SlicesState& p) {
+    return p.kind == SLICE_INJECT ? "slice injectors" : p.kind == SLICE_CORRELATE ? "slice correlators" : "slice recorders";
 }
 
 bool active(const SlicesState* p) { return p && !p->recs.empty(); }
 
-// this rank's part of one recorder or injector; refuses a box outside the overall domain, and on a rank grid an injector into a
-// var the last stage does not write (it must land before that stage's exchange, as a source does)
+// A consumer of a recorder's frames against the recorder (FrameLink): the same box and stride, at most its rows, and the same
+// owned part of the box on this rank -- the same overall domain, rank grid and rank index -- on the same device.  Each refusal
+// names the field that differs.
+int check_link(const Solution& s, const SlicesState& p, const SliceRec& r) {
+    const FrameLink& l = *r.link;
+    const long long id = l.src_id;
+    for (int k = 0; k < s.ndd; k++) {
+        const char* dn = s.spec.domain_dims[k].c_str();
+        if (r.first[k] != l.first[k] || r.last[k] != l.last[k])
+            return set_error(YB_EINVAL, "%s: box [%lld, %lld] in dim '%s' differs from recorder %lld's box [%lld, %lld]", p.what, (long long)r.first[k],
+                             (long long)r.last[k], dn, id, (long long)l.first[k], (long long)l.last[k]);
+        if (r.stride[k] != l.stride[k])
+            return set_error(YB_EINVAL, "%s: stride %lld in dim '%s' differs from recorder %lld's stride %lld", p.what, (long long)r.stride[k], dn,
+                             id, (long long)l.stride[k]);
+    }
+    if (r.nrows > l.nrows)
+        return set_error(YB_EINVAL, "%s: nrows = %lld is more than the %lld rows of recorder %lld", p.what, (long long)r.nrows, (long long)l.nrows, id);
+    if (!geometry_known(s)) return 0;           // checked again at plan_geometry / prepare
+    for (int k = 0; k < s.ndd; k++) {
+        const char* dn = s.spec.domain_dims[k].c_str();
+        if (s.overall_size[k] != l.overall[k])
+            return set_error(YB_EINVAL, "%s: overall domain size %lld in dim '%s' differs from the source solution's %lld", p.what,
+                             (long long)s.overall_size[k], dn, (long long)l.overall[k]);
+        if (s.num_ranks[k] != l.num_ranks[k])
+            return set_error(YB_EINVAL, "%s: num_ranks %lld in dim '%s' differs from the source solution's %lld (rank grid)", p.what,
+                             (long long)s.num_ranks[k], dn, (long long)l.num_ranks[k]);
+        if (s.rank_index[k] != l.rank_index[k])
+            return set_error(YB_EINVAL, "%s: rank index %lld in dim '%s' differs from the source solution's %lld", p.what,
+                             (long long)s.rank_index[k], dn, (long long)l.rank_index[k]);
+        if (r.own_k0[k] != l.own_k0[k] || r.own_n[k] != l.own_n[k])
+            return set_error(YB_EINVAL, "%s: owned part (first %lld, count %lld) in dim '%s' differs from recorder %lld's (first %lld, count %lld)",
+                             p.what, (long long)r.own_k0[k], (long long)r.own_n[k], dn, id, (long long)l.own_k0[k], (long long)l.own_n[k]);
+    }
+    if (s.device >= 0 && s.device != l.device)
+        return set_error(YB_EINVAL, "%s: device %d differs from the source solution's device %d", p.what, s.device, l.device);
+    return 0;
+}
+
+// this rank's part of one recorder, injector or correlator; refuses a box outside the overall domain, on a rank grid an injector
+// into a var the last stage does not write (it must land before that stage's exchange, as a source does), and a consumer whose
+// part differs from its recorder's (check_link)
 int plan_one(const Solution& s, const SlicesState& p, SliceRec& r) {
     const Var& v = s.vars[r.var];
-    if (p.inject && s.multi_rank()) {
+    if (p.kind == SLICE_INJECT && s.multi_rank()) {
         bool last = false;
         for (int o : s.spec.stages.back().outputs) last = last || o == r.var;
         if (!last)
@@ -149,11 +252,18 @@ int plan_one(const Solution& s, const SlicesState& p, SliceRec& r) {
         const Dim* d = v.domain_dim(k);
         r.own_off += (r.first[k] + k0 * st - lo + d->pad_l) * d->stride;
     }
-    return 0;
+    return r.link ? check_link(s, p, r) : 0;
 }
 
 // rank-local coordinate of the first owned point in domain dim k (the last one is that + (own_n[k] - 1) * stride[k])
 int64_t own_loc0(const Solution& s, const SliceRec& r, int k) { return r.first[k] + r.own_k0[k] * r.stride[k] - s.rank_offset[k]; }
+
+// a correlator's threads per row of the unit-stride dim of `len` points: the power of two at or above it, up to the CTA's 256
+int lanes_log2(int64_t len) {
+    int lg = 0;
+    while (lg < 8 && (int64_t(1) << lg) < len) lg++;
+    return lg;
+}
 
 SliceDesc describe(const Solution& s, const SliceRec& r) {
     const Var& v = s.vars[r.var];
@@ -175,11 +285,12 @@ SliceDesc describe(const Solution& s, const SliceRec& r) {
         d.loc0[4 - s.ndd + k] = own_loc0(s, r, k);
         d.lstep[4 - s.ndd + k] = r.stride[k];
     }
-    d.frames = static_cast<char*>(r.d_frames);
+    d.frames = static_cast<char*>(r.frames.get());
+    d.image = static_cast<char*>(r.image.get());
+    d.rev = r.rev;
+    d.lanes_log2 = lanes_log2(d.box.n[3]);
     return d;
 }
-
-size_t frame_bytes(const Solution& s, const SliceRec& r) { return size_t(r.nrows) * size_t(r.own_elems) * s.spec.elem_bytes; }
 
 // The owned part of `rows` rows of the whole decimated box as contiguous runs of the last dim: f(element index of the run in
 // rows x the whole box, its index in rows x the owned part, length).
@@ -195,29 +306,38 @@ void owned_runs(const Solution& s, const SliceRec& r, int64_t rows, F f) {
 }
 
 // Recorders: zeroed frames.  Injectors: this rank's part of the caller's frames, after which the host copy is dropped (the
-// geometry is fixed once a solution is prepared).
+// geometry is fixed once a solution is prepared); one fed from a recorder holds that recorder's frames already.  Correlators: a
+// zeroed image of one frame (their source frames, if any, are a recorder's).
 int alloc_frames(const Solution& s, const SlicesState& p, SliceRec& r) {
-    const size_t bytes = frame_bytes(s, r);
-    if (r.d_frames) return 0;
+    const bool corr = p.kind == SLICE_CORRELATE;
+    std::shared_ptr<void>& buf = corr ? r.image : r.frames;
+    const int64_t rows = corr ? 1 : r.nrows;
+    const size_t bytes = size_t(rows) * size_t(r.own_elems) * s.spec.elem_bytes;
+    if (buf || (r.link && !corr)) return 0;
     if (!bytes) {
         std::vector<char>().swap(r.host_frames);
         return 0;
     }
-    cudaError_t e = cudaMalloc(&r.d_frames, bytes);
+    void* d = nullptr;
+    cudaError_t e = cudaMalloc(&d, bytes);
     if (e != cudaSuccess) {
         (void)cudaGetLastError();
-        r.d_frames = nullptr;
-        return set_error(YB_ENOMEM, "%s: cannot allocate %zu bytes of frames (%lld rows x %lld owned points) on device %d: %s", p.what, bytes,
-                         (long long)r.nrows, (long long)r.own_elems, s.device, cudaGetErrorString(e));
+        return set_error(YB_ENOMEM, "%s: cannot allocate %zu bytes of %s (%lld rows x %lld owned points) on device %d: %s", p.what, bytes,
+                         corr ? "image" : "frames", (long long)rows, (long long)r.own_elems, s.device, cudaGetErrorString(e));
     }
-    if (!p.inject) {
-        YB_CUDA(cudaMemset(r.d_frames, 0, bytes));
+    try {
+        buf = device_buffer(d, s.device);
+    } catch (const std::exception&) {
+        return set_error(YB_ENOMEM, "%s: cannot hold %zu bytes of device memory", p.what, bytes);
+    }
+    if (p.kind != SLICE_INJECT) {
+        YB_CUDA(cudaMemset(d, 0, bytes));
         return 0;
     }
     const size_t eb = size_t(s.spec.elem_bytes);
     std::vector<char> dense(bytes);
     owned_runs(s, r, r.nrows, [&](size_t whole, size_t own, size_t n) { memcpy(dense.data() + own * eb, r.host_frames.data() + whole * eb, n * eb); });
-    YB_CUDA(cudaMemcpy(r.d_frames, dense.data(), bytes, cudaMemcpyHostToDevice));
+    YB_CUDA(cudaMemcpy(d, dense.data(), bytes, cudaMemcpyHostToDevice));
     std::vector<char>().swap(r.host_frames);
     return 0;
 }
@@ -267,7 +387,7 @@ int check_mode(const Solution& s, const SlicesState& p) {
     if (fused_pair_rank_grid(s))
         return set_error(YB_EUNSUPPORTED, "%s are not supported on a rank grid in fused-pair mode (block_steps=2 with "
                                           "mega_block_steps=2): its halos are exchanged once per pair of steps, and the state after the first "
-                                          "step of a pair is never stored", p.inject ? "slice injectors" : "slice recorders");
+                                          "step of a pair is never stored", plural(p));
     return 0;
 }
 
@@ -319,30 +439,69 @@ void slices_free(SlicesState* p) {
     delete p;
 }
 
+FrameLink::~FrameLink() {
+    if (!written && !read) return;
+    int cur = -1;
+    const bool had = cudaGetDevice(&cur) == cudaSuccess;
+    cudaSetDevice(device);
+    if (written) cudaEventDestroy(written);
+    if (read) cudaEventDestroy(read);
+    if (had) cudaSetDevice(cur);
+}
+
 void slices_preload() {
     preload_kernel((const void*)slices_kernel<float>);
     preload_kernel((const void*)slices_kernel<double>);
     preload_kernel((const void*)slice_injectors_kernel<float>);
     preload_kernel((const void*)slice_injectors_kernel<double>);
+    preload_kernel((const void*)slice_correlators_kernel<float>);
+    preload_kernel((const void*)slice_correlators_kernel<double>);
 }
 
 bool slices_active(const Solution& s) { return active(s.slices); }
 
 bool slice_injectors_active(const Solution& s) { return active(s.injectors); }
 
+bool slice_correlators_active(const Solution& s) { return active(s.correlators); }
+
 int slices_plan(Solution& s) {
-    if (int rc = plan_state(s, s.slices)) return rc;
-    return plan_state(s, s.injectors);
+    for (SlicesState* p : {s.slices, s.injectors, s.correlators})
+        if (int rc = plan_state(s, p)) return rc;
+    return 0;
 }
 
 int slices_prepare(Solution& s) {
-    if (int rc = prepare_state(s, s.slices)) return rc;
-    return prepare_state(s, s.injectors);
+    for (SlicesState* p : {s.slices, s.injectors, s.correlators})
+        if (int rc = prepare_state(s, p)) return rc;
+    return 0;
 }
 
 int slices_begin_run(Solution& s) {
-    if (int rc = begin_run_state(s, s.slices)) return rc;
-    return begin_run_state(s, s.injectors);
+    for (SlicesState* p : {s.slices, s.injectors, s.correlators})
+        if (int rc = begin_run_state(s, p)) return rc;
+    return 0;
+}
+
+int slices_run_waits(Solution& s, cudaStream_t st) {
+    for (SlicesState* p : {s.injectors, s.correlators})
+        if (active(p))
+            for (const SliceRec& r : p->recs)
+                if (r.link && r.link->written) YB_CUDA(cudaStreamWaitEvent(st, r.link->written, 0));
+    if (s.slices)
+        for (const auto& w : s.slices->readers)
+            if (auto l = w.lock()) YB_CUDA(cudaStreamWaitEvent(st, l->read, 0));
+    return 0;
+}
+
+int slices_run_records(Solution& s, cudaStream_t st) {
+    for (SlicesState* p : {s.injectors, s.correlators})
+        if (active(p))
+            for (const SliceRec& r : p->recs)
+                if (r.link && r.link->read) YB_CUDA(cudaEventRecord(r.link->read, st));
+    if (s.slices)
+        for (const auto& w : s.slices->readers)
+            if (auto l = w.lock()) YB_CUDA(cudaEventRecord(l->written, st));
+    return 0;
 }
 
 int slices_launch(Solution& s, int64_t t, cudaStream_t st) {
@@ -358,6 +517,27 @@ int slices_launch(Solution& s, int64_t t, cudaStream_t st) {
     const SliceDesc* table = static_cast<const SliceDesc*>(p.d_table);
     if (s.spec.elem_bytes == 4) slices_kernel<float><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
     else slices_kernel<double><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
+    YB_CUDA(cudaGetLastError());
+    p.launches++;
+    return 1;
+}
+
+int slice_correlators_launch(Solution& s, int64_t t, cudaStream_t st) {
+    if (!slice_correlators_active(s)) return 0;
+    SlicesState& p = *s.correlators;
+    int64_t most = 0;
+    for (auto& r : p.recs) {
+        long long row;
+        if (!r.own_elems || !row_due(t + r.step_off, r.t0, r.every, r.nrows, row)) continue;
+        // the CTAs this correlator's rows fill, 256 >> lanes_log2 rows per CTA
+        const int64_t len = r.own_n[s.ndd - 1], per = 256 >> lanes_log2(len);
+        most = std::max(most, (r.own_elems / len + per - 1) / per);
+    }
+    if (!most) return 0;
+    const dim3 grid(unsigned(std::min<int64_t>(most, int64_t(p.num_sms) * CTAS_PER_SM)), unsigned(std::min<size_t>(p.recs.size(), MAX_GRID_Y)));
+    const SliceDesc* table = static_cast<const SliceDesc*>(p.d_table);
+    if (s.spec.elem_bytes == 4) slice_correlators_kernel<float><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
+    else slice_correlators_kernel<double><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
     YB_CUDA(cudaGetLastError());
     p.launches++;
     return 1;
@@ -452,10 +632,11 @@ static int new_rec(Solution* s, const char* what, const char* var, const int64_t
     return 0;
 }
 
-// Append r to *pp (created on first use): planned now when the rank geometry is known; on a prepared solution its frames are
-// allocated and the table uploaded now too -- never by run_solution() -- after the work that may read the old table.
-static int install(Solution* s, SlicesState*& pp, bool inject, SliceRec&& r, int64_t* id) {
-    if (!pp) pp = new_state(inject);
+// Append r to *pp (created on first use): planned now when the rank geometry is known; on a prepared solution its frames (a
+// correlator's image) are allocated and the table uploaded now too -- never by run_solution() -- after the work that may read the
+// old table.
+static int install(Solution* s, SlicesState*& pp, SliceKind kind, SliceRec&& r, int64_t* id) {
+    if (!pp) pp = new_state(kind);
     SlicesState& p = *pp;
     if (geometry_known(*s)) {
         if (int rc = check_mode(*s, p)) return rc;
@@ -474,12 +655,63 @@ static int install(Solution* s, SlicesState*& pp, bool inject, SliceRec&& r, int
     } else {
         p.recs.push_back(std::move(r));
     }
-    if (inject) plan_groups(p);
+    if (kind == SLICE_INJECT) plan_groups(p);
     if (id) *id = int64_t(p.recs.size()) - 1;
     return 0;
 }
 
-static int clear_state(Solution* s, SlicesState*& p, bool inject) {
+// Point r (its box and window filled by new_rec) at the frames of recorder src_id of solution src, read in forward or reversed
+// row order.  Every check but the source's frames is made first, so that a planned source shows each refusal; then r holds the
+// frames, and when src is another solution, the events that order the two streams (created here: run_solution() allocates
+// nothing).
+static int attach(Solution* s, SlicesState*& pp, SliceKind kind, SliceRec& r, yb_solution* src_, int64_t src_id, int reverse) {
+    if (!pp) pp = new_state(kind);
+    const SlicesState& p = *pp;
+    if (reverse != 0 && reverse != 1) return set_error(YB_EINVAL, "%s: reverse = %d is not 0 or 1", p.what, reverse);
+    r.rev = reverse;
+    Solution* src = SOL(src_);
+    if (!src) return set_error(YB_EINVAL, "%s: null source solution", p.what);
+    if (!slices_active(*src) || src_id < 0 || src_id >= int64_t(src->slices->recs.size()))
+        return set_error(YB_EINVAL, "%s: src_id %lld is not a slice recorder of the source solution '%s'", p.what, (long long)src_id,
+                         src->spec.name.c_str());
+    if (src->spec.elem_bytes != s->spec.elem_bytes)
+        return set_error(YB_EINVAL, "%s: element bytes %d differ from the source solution's %d", p.what, s->spec.elem_bytes, src->spec.elem_bytes);
+    if (src->ndd != s->ndd)
+        return set_error(YB_EINVAL, "%s: %d domain dims differ from the source solution's %d", p.what, s->ndd, src->ndd);
+    if (!geometry_known(*s)) return set_error(YB_ESTATE, "%s: this solution has no rank geometry yet (plan_geometry / prepare_solution)", p.what);
+    if (!geometry_known(*src))
+        return set_error(YB_ESTATE, "%s: the source solution has no rank geometry yet (plan_geometry / prepare_solution)", p.what);
+    const SliceRec& q = src->slices->recs[size_t(src_id)];
+    auto link = std::make_shared<FrameLink>();
+    link->device = src->device;
+    link->elem_bytes = src->spec.elem_bytes;
+    link->ndd = src->ndd;
+    link->src_id = src_id;
+    link->nrows = q.nrows;
+    for (int k = 0; k < 3; k++) {
+        link->first[k] = q.first[k]; link->last[k] = q.last[k]; link->stride[k] = q.stride[k];
+        link->overall[k] = src->overall_size[k]; link->num_ranks[k] = src->num_ranks[k]; link->rank_index[k] = src->rank_index[k];
+        link->own_k0[k] = q.own_k0[k]; link->own_n[k] = q.own_n[k];
+    }
+    r.link = link;
+    if (int rc = check_mode(*s, p)) return rc;
+    if (int rc = plan_one(*s, p, r)) return rc;
+    if (!src->prepared)
+        return set_error(YB_ESTATE, "%s: the source solution '%s' is not prepared, so recorder %lld has no frames yet", p.what,
+                         src->spec.name.c_str(), (long long)src_id);
+    r.frames = q.frames;
+    if (src == s) return 0;                     // one stream
+    YB_CUDA(cudaSetDevice(src->device));
+    YB_CUDA(cudaEventCreateWithFlags(&link->written, cudaEventDisableTiming));
+    YB_CUDA(cudaEventCreateWithFlags(&link->read, cudaEventDisableTiming));
+    YB_CUDA(cudaEventRecord(link->written, src->stream()));     // the source's runs enqueued so far
+    auto& readers = src->slices->readers;
+    readers.erase(std::remove_if(readers.begin(), readers.end(), [](const std::weak_ptr<FrameLink>& w) { return w.expired(); }), readers.end());
+    readers.push_back(link);
+    return 0;
+}
+
+static int clear_state(Solution* s, SlicesState*& p, SliceKind kind) {
     if (!p) return 0;
     if (s->prepared) {
         YB_CUDA(cudaSetDevice(s->device));
@@ -487,8 +719,29 @@ static int clear_state(Solution* s, SlicesState*& p, bool inject) {
     }
     const int64_t launches = p->launches;
     slices_free(p);
-    p = new_state(inject);
+    p = new_state(kind);
     p->launches = launches;
+    return 0;
+}
+
+// `rows` rows of the whole decimated box of r into out from `dev` (rows x this rank's part; null when nothing was allocated), 0
+// where this rank owns no point, and the owned mask.  `out` may be null: the mask only, which needs no device.
+static int copy_out(Solution* s, const SliceRec& r, const void* dev, int64_t rows, void* out, uint8_t* owned) {
+    size_t box = 1;
+    for (int k = 0; k < s->ndd; k++) box *= size_t(r.count[k]);
+    if (owned) {
+        memset(owned, 0, box);
+        owned_runs(*s, r, 1, [&](size_t whole, size_t, size_t n) { memset(owned + whole, 1, n); });
+    }
+    if (!out) return 0;
+    const size_t eb = size_t(s->spec.elem_bytes);
+    memset(out, 0, size_t(rows) * box * eb);
+    if (!dev) return 0;
+    std::vector<char> dense(size_t(rows) * size_t(r.own_elems) * eb);
+    YB_CUDA(cudaSetDevice(s->device));
+    YB_CUDA(cudaMemcpyAsync(dense.data(), dev, dense.size(), cudaMemcpyDeviceToHost, s->stream()));
+    YB_CUDA(cudaStreamSynchronize(s->stream()));
+    owned_runs(*s, r, rows, [&](size_t whole, size_t own, size_t n) { memcpy(static_cast<char*>(out) + whole * eb, dense.data() + own * eb, n * eb); });
     return 0;
 }
 
@@ -501,7 +754,7 @@ int yb_solution_add_slice(yb_solution* s_, const char* var, const int64_t* first
     SliceRec r;
     int64_t bytes = 0;
     if (int rc = new_rec(s, "slice", var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
-    return install(s, s->slices, false, std::move(r), id);
+    return install(s, s->slices, SLICE_RECORD, std::move(r), id);
 }
 
 int yb_solution_add_slice_injector(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
@@ -521,7 +774,38 @@ int yb_solution_add_slice_injector(yb_solution* s_, const char* var, const int64
     } catch (const std::exception&) {
         return set_error(YB_ENOMEM, "%s: cannot copy %lld bytes of frames on the host", what, (long long)bytes);
     }
-    return install(s, s->injectors, true, std::move(r), id);
+    return install(s, s->injectors, SLICE_INJECT, std::move(r), id);
+}
+
+int yb_solution_add_slice_injector_from(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                        int64_t t0, int64_t every, int64_t nrows, int mode, yb_solution* src, int64_t src_id, int reverse,
+                                        int64_t* id) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    const char* what = "slice injector";
+    SliceRec r;
+    int64_t bytes = 0;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (mode != YB_INJECT_ADD && mode != YB_INJECT_SET)
+        return set_error(YB_EINVAL, "%s: unknown mode %d (YB_INJECT_ADD = %d or YB_INJECT_SET = %d)", what, mode, YB_INJECT_ADD, YB_INJECT_SET);
+    r.mode = mode;
+    if (int rc = attach(s, s->injectors, SLICE_INJECT, r, src, src_id, reverse)) return rc;
+    return install(s, s->injectors, SLICE_INJECT, std::move(r), id);
+}
+
+int yb_solution_add_slice_correlator(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                     int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    SliceRec r;
+    int64_t bytes = 0;
+    if (int rc = new_rec(s, "slice correlator", var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (src) {
+        if (int rc = attach(s, s->correlators, SLICE_CORRELATE, r, src, src_id, reverse)) return rc;
+    } else if (reverse != 0 && reverse != 1) {
+        return set_error(YB_EINVAL, "slice correlator: reverse = %d is not 0 or 1", reverse);
+    }
+    return install(s, s->correlators, SLICE_CORRELATE, std::move(r), id);
 }
 
 int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t* owned) {
@@ -533,34 +817,37 @@ int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t
     SliceRec& r = s->slices->recs[size_t(id)];
     if (!s->prepared)
         if (int rc = plan_one(*s, *s->slices, r)) return rc;
-    size_t box = 1;
-    for (int k = 0; k < s->ndd; k++) box *= size_t(r.count[k]);
-    if (owned) {
-        memset(owned, 0, box);
-        owned_runs(*s, r, 1, [&](size_t whole, size_t, size_t n) { memset(owned + whole, 1, n); });
-    }
-    if (!out) return 0;
-    const size_t eb = size_t(s->spec.elem_bytes);
-    memset(out, 0, size_t(r.nrows) * box * eb);
-    if (!r.d_frames) return 0;
-    std::vector<char> dense(frame_bytes(*s, r));
-    YB_CUDA(cudaSetDevice(s->device));
-    YB_CUDA(cudaMemcpyAsync(dense.data(), r.d_frames, dense.size(), cudaMemcpyDeviceToHost, s->stream()));
-    YB_CUDA(cudaStreamSynchronize(s->stream()));
-    owned_runs(*s, r, r.nrows, [&](size_t whole, size_t own, size_t n) { memcpy(static_cast<char*>(out) + whole * eb, dense.data() + own * eb, n * eb); });
-    return 0;
+    return copy_out(s, r, r.frames.get(), r.nrows, out, owned);
+}
+
+int yb_solution_get_correlator_image(yb_solution* s_, int64_t id, void* out, uint8_t* owned) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    if (!slice_correlators_active(*s) || id < 0 || id >= int64_t(s->correlators->recs.size()))
+        return set_error(YB_EINVAL, "get_correlator_image: no slice correlator %lld", (long long)id);
+    if (!geometry_known(*s)) return set_error(YB_ESTATE, "get_correlator_image: the rank geometry is not known yet (plan_geometry / prepare_solution)");
+    SliceRec& r = s->correlators->recs[size_t(id)];
+    if (!s->prepared)
+        if (int rc = plan_one(*s, *s->correlators, r)) return rc;
+    return copy_out(s, r, r.image.get(), 1, out, owned);
 }
 
 int yb_solution_clear_slices(yb_solution* s_) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
-    return clear_state(s, s->slices, false);
+    return clear_state(s, s->slices, SLICE_RECORD);
 }
 
 int yb_solution_clear_slice_injectors(yb_solution* s_) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
-    return clear_state(s, s->injectors, true);
+    return clear_state(s, s->injectors, SLICE_INJECT);
+}
+
+int yb_solution_clear_slice_correlators(yb_solution* s_) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    return clear_state(s, s->correlators, SLICE_CORRELATE);
 }
 
 }  // extern "C"

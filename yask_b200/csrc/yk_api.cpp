@@ -482,6 +482,7 @@ struct B200Solution : yk_solution {
     int device = -1;
     idx_t point_rcv = 0, point_rows = 0;   // shape of the receiver set (yk_set_receivers)
     std::vector<idx_t_vec> slice_shape;     // frames shape (nrows, box extents...) of each slice recorder (yk_add_slice)
+    std::vector<idx_t_vec> correlator_shape;   // image shape (box extents...) of each slice correlator (yk_add_slice_correlator)
 
     // The reference fixes a solution's radius and element size when it builds the kernel library (`make stencil=iso3dfd
     // radius=2 real_bytes=8`, /root/reference/src/kernel/Makefile); here the library name carries them the same way:
@@ -1031,6 +1032,73 @@ void yk_clear_slice_injectors(yk_solution_ptr soln) { chk(yb_solution_clear_slic
 idx_t yk_get_slice_injector_launches(yk_solution_ptr soln) {
     char v[64];
     chk(yb_get_option(b200_slices(soln).h->s, "slice_injector_launches", v, sizeof v));
+    return idx_t(atoll(v));
+}
+
+namespace {
+// the C ABI's box arguments of a slice call, checked against the solution's domain dims
+void slice_box(B200Solution& s, const char* what, const idx_t_vec& first, const idx_t_vec& last, const idx_t_vec& stride,
+               std::vector<int64_t>& f, std::vector<int64_t>& l, std::vector<int64_t>& st) {
+    const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
+    if (first.size() != nd || last.size() != nd || (!stride.empty() && stride.size() != nd))
+        fail(std::string(what) + ": first, last and stride need " + std::to_string(nd) + " domain indices each");
+    f.assign(first.begin(), first.end());
+    l.assign(last.begin(), last.end());
+    st.assign(stride.begin(), stride.end());
+}
+}  // namespace
+
+idx_t yk_add_slice_injector_from(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                 idx_t nrows, yk_solution_ptr src, idx_t src_id, bool reverse, const idx_t_vec& stride, idx_t every, bool set) {
+    B200Solution& s = b200_slices(soln);
+    std::vector<int64_t> f, l, st;
+    slice_box(s, "slice injector", first, last, stride, f, l, st);
+    int64_t id = -1;
+    chk(yb_solution_add_slice_injector_from(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows,
+                                            set ? YB_INJECT_SET : YB_INJECT_ADD, b200_slices(src).h->s, src_id, reverse ? 1 : 0, &id));
+    return idx_t(id);
+}
+
+idx_t yk_add_slice_correlator(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                              idx_t nrows, yk_solution_ptr src, idx_t src_id, bool reverse, const idx_t_vec& stride, idx_t every) {
+    B200Solution& s = b200_slices(soln);
+    std::vector<int64_t> f, l, st;
+    slice_box(s, "slice correlator", first, last, stride, f, l, st);
+    int64_t id = -1;
+    chk(yb_solution_add_slice_correlator(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows,
+                                         src ? b200_slices(src).h->s : nullptr, src_id, reverse ? 1 : 0, &id));
+    idx_t_vec shape;
+    for (size_t k = 0; k < f.size(); k++) shape.push_back((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1);
+    s.correlator_shape.resize(size_t(id) + 1);
+    s.correlator_shape[size_t(id)] = shape;
+    return idx_t(id);
+}
+
+void yk_get_correlator_image(yk_solution_ptr soln, idx_t id, std::vector<double>& image, idx_t_vec& shape, std::vector<bool>& owned) {
+    B200Solution& s = b200_slices(soln);
+    if (id < 0 || size_t(id) >= s.correlator_shape.size()) fail("get_correlator_image: no slice correlator " + std::to_string(id));
+    shape = s.correlator_shape[size_t(id)];
+    size_t n = 1;
+    for (idx_t e : shape) n *= size_t(e);
+    const int eb = yb_solution_elem_bytes(s.h->s);
+    std::vector<char> raw(n * eb);
+    std::vector<uint8_t> own(n);
+    chk(yb_solution_get_correlator_image(s.h->s, id, yb_solution_is_prepared(s.h->s) ? raw.data() : nullptr, own.data()));
+    image.resize(n);
+    for (size_t i = 0; i < n; i++)
+        image[i] = eb == 4 ? double(reinterpret_cast<const float*>(raw.data())[i]) : reinterpret_cast<const double*>(raw.data())[i];
+    owned.assign(own.begin(), own.end());
+}
+
+void yk_clear_slice_correlators(yk_solution_ptr soln) {
+    B200Solution& s = b200_slices(soln);
+    chk(yb_solution_clear_slice_correlators(s.h->s));
+    s.correlator_shape.clear();
+}
+
+idx_t yk_get_slice_correlator_launches(yk_solution_ptr soln) {
+    char v[64];
+    chk(yb_get_option(b200_slices(soln).h->s, "slice_correlator_launches", v, sizeof v));
     return idx_t(atoll(v));
 }
 

@@ -322,4 +322,20 @@ PYBIND11_MODULE(yask_kernel, m) {
           py::arg("nrows"), py::arg("frames"), py::arg("stride") = idx_t_vec{}, py::arg("every") = 1, py::arg("set") = false);
     m.def("yk_clear_slice_injectors", &yk_clear_slice_injectors, py::arg("soln"));
     m.def("yk_get_slice_injector_launches", &yk_get_slice_injector_launches, py::arg("soln"));
+    m.def("yk_add_slice_injector_from", &yk_add_slice_injector_from, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
+          py::arg("t0"), py::arg("nrows"), py::arg("src"), py::arg("src_id"), py::arg("reverse") = false, py::arg("stride") = idx_t_vec{},
+          py::arg("every") = 1, py::arg("set") = false);
+    // ---- slice correlators on the device (yask_b200_slices.hpp; not in the reference API) ----
+    m.def("yk_add_slice_correlator", &yk_add_slice_correlator, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
+          py::arg("t0"), py::arg("nrows"), py::arg("src") = yk_solution_ptr(), py::arg("src_id") = 0, py::arg("reverse") = false,
+          py::arg("stride") = idx_t_vec{}, py::arg("every") = 1);
+    m.def("yk_get_correlator_image", [](yk_solution_ptr s, idx_t id) {
+        std::vector<double> image;
+        idx_t_vec shape;
+        std::vector<bool> owned;
+        yk_get_correlator_image(s, id, image, shape, owned);
+        return py::make_tuple(image, shape, owned);
+    }, py::arg("soln"), py::arg("id"), "(image as a flat list of floats, shape (box extents...), owned per box point)");
+    m.def("yk_clear_slice_correlators", &yk_clear_slice_correlators, py::arg("soln"));
+    m.def("yk_get_slice_correlator_launches", &yk_get_slice_correlator_launches, py::arg("soln"));
 }

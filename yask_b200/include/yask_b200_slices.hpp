@@ -1,4 +1,4 @@
-// Slice recorders and injectors on the device inside run_solution(): an extension of the C++ kernel API of this engine.
+// Slice recorders, injectors and correlators on the device inside run_solution(): an extension of the C++ kernel API of this engine.
 //
 // The reference API has no such calls; its users record a receiver plane or a snapshot from the host, one step at a time:
 //
@@ -44,5 +44,30 @@ idx_t yk_add_slice_injector(yk_solution_ptr soln, const std::string& var, const 
 void yk_clear_slice_injectors(yk_solution_ptr soln);
 // Injecting launches since prepare_solution().
 idx_t yk_get_slice_injector_launches(yk_solution_ptr soln);
+// An injector whose frames are those of recorder src_id of solution src (which may be soln), read on the device with no copy: row
+// r reads recorder row nrows - 1 - r when reverse, else r.  Checks, sharing and ordering: yb_solution_add_slice_correlator.
+idx_t yk_add_slice_injector_from(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                 idx_t nrows, yk_solution_ptr src, idx_t src_id, bool reverse = false, const idx_t_vec& stride = {},
+                                 idx_t every = 1, bool set = false);
+
+// Slice correlators, the imaging condition of a reverse-time shot: replaces the host loop
+//
+//     soln->run_solution(t);  p->get_elements_in_slice(box, ...);  image += frame[r] * box[::stride];
+//
+// After every step u a run computes, if u - t0 is a multiple of `every` and r = (u - t0) / every < nrows, image += var(u) * b at
+// first[d], first[d] + stride[d], ... <= last[d], the product and the sum each rounded to the element type, after that step's
+// recorders.  b is var(u) when src is null (the illumination), else row r (nrows - 1 - r when reverse) of recorder src_id of src
+// (which may be soln).  Semantics and checks: yb_solution_add_slice_correlator in include/yask_b200.h.  Returns the correlator's
+// id (0, 1, ... until yk_clear_slice_correlators; separate from the recorders' and injectors').
+idx_t yk_add_slice_correlator(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                              idx_t nrows, yk_solution_ptr src = nullptr, idx_t src_id = 0, bool reverse = false,
+                              const idx_t_vec& stride = {}, idx_t every = 1);
+// image: the decimated box, row-major, the last domain dim fastest, widened to double (points this rank does not own are 0);
+// shape: the box extents; owned: per box point, this rank holds it.
+void yk_get_correlator_image(yk_solution_ptr soln, idx_t id, std::vector<double>& image, idx_t_vec& shape, std::vector<bool>& owned);
+// Remove every correlator and free its image.
+void yk_clear_slice_correlators(yk_solution_ptr soln);
+// Correlating launches since prepare_solution().
+idx_t yk_get_slice_correlator_launches(yk_solution_ptr soln);
 
 }  // namespace yask
