@@ -254,11 +254,19 @@ struct IsoSpongeRegs {
     E z[IsoVec<E>::N];      // cr_z of the thread's vector
 };
 
-template <class T, int MODE, int B, int QL, bool SP = false>
+// Default `pv_load` of iso_rows_update: the caller waited for the p(t-1) and v tiles before the call.
+struct IsoPvLoaded {
+    template <class F>
+    __device__ __forceinline__ void operator()(F&& load) const { load(); }
+};
+
+// pv_load(load) runs load(), the reads of the p(t-1) and v vectors.  They come after the stencil sums, so a caller that has
+// not yet waited for those tiles can wait inside pv_load, with the sums' arithmetic as cover for the load.
+template <class T, int MODE, int B, int QL, bool SP = false, class PvLoad = IsoPvLoaded>
 __device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>& P, const typename T::V (&qa)[QL],
                                                 const typename T::V (&qb)[QL], const uint8_t* h, const uint8_t* pv,
                                                 const uint8_t* v, typename T::E* oa, int xo, int nva, int nvb, bool vec_ok,
-                                                const IsoSpongeRegs<typename T::E>* sg = nullptr) {
+                                                const IsoSpongeRegs<typename T::E>* sg = nullptr, PvLoad pv_load = {}) {
     using E = typename T::E;
     using V = typename T::V;
     constexpr int R = T::R, ZQ = T::ZQ, VW = T::VW, ES = T::ES;
@@ -312,10 +320,12 @@ __device__ __forceinline__ void iso_rows_update(const IsoParamsT<typename T::E>&
             for (int i = 0; i < VW; i++) { wlo_prev[i] = wlo[i]; whi_prev[i] = whi[i]; }
         }
         E pva[VW], vva[VW], pvb[VW], vvb[VW], ea[VW], eb[VW];
-        f4_to_arr(*reinterpret_cast<const V*>(pv), pva);
-        f4_to_arr(*reinterpret_cast<const V*>(v), vva);
-        f4_to_arr(*reinterpret_cast<const V*>(pv + T::TZ * ES), pvb);
-        f4_to_arr(*reinterpret_cast<const V*>(v + T::TZ * ES), vvb);
+        pv_load([&] {
+            f4_to_arr(*reinterpret_cast<const V*>(pv), pva);
+            f4_to_arr(*reinterpret_cast<const V*>(v), vva);
+            f4_to_arr(*reinterpret_cast<const V*>(pv + T::TZ * ES), pvb);
+            f4_to_arr(*reinterpret_cast<const V*>(v + T::TZ * ES), vvb);
+        });
 #pragma unroll
         for (int i = 0; i < VW; i++) ea[i] = iso_final<MODE>(acca[i], pa[i], pva[i], vva[i]);
 #pragma unroll
@@ -658,9 +668,12 @@ iso3dfd_tma3_kernel(const __grid_constant__ IsoMaps M, const __grid_constant__ I
             const int hc = hs >= R ? hs - R : hs - R + NS;     // slot of the plane computed now
             if (compute) {
                 const uint8_t* pv = sbase + T::PV_OFF + ps * T::PV_BYTES;
-                mbar_wait(&pv_full[ps], pph);
+                // p(t-1) and v are first read by iso_final, after the stencil sums: wait for them there, so the sums cover
+                // their load.  The memory probe (MODE 3) reads them first and keeps the wait it is measured with.
+                if constexpr (MODE == 3) mbar_wait(&pv_full[ps], pph);
                 iso_rows_update<T, MODE, B>(P, qa, qb, sbase + hc * T::SLOT_BYTES + h_own, pv + c_own, pv + T::C_BYTES + c_own,
-                                            out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb, vec_ok);
+                                            out_a + (long long)(it - 2 * R) * out_step, cu.x0 + cu.dir * (it - 2 * R), nva, nvb, vec_ok,
+                                            nullptr, [&](auto&& load) { mbar_wait(&pv_full[ps], pph); load(); });
             }
             __syncwarp();
             if (lane == 0) {
