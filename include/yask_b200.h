@@ -341,6 +341,39 @@ int yb_solution_add_slice_correlator(yb_solution* s, const char* var, const int6
 int yb_solution_get_correlator_image(yb_solution* s, int64_t id, void* out, uint8_t* owned);
 int yb_solution_clear_slice_correlators(yb_solution* s);   /* remove every correlator and free its image; ids restart at 0 */
 
+/* ---- frame and image types of the slice calls ------------------------------------------------------------------------
+ * A recorder's or a host-fed injector's frames are held in a frame type F, and a correlator's image in an image type I.
+ * YB_TYPE_ELEM (the default of the untyped calls) is the solution's element type T, and leaves every bit, allocation, launch and
+ * counter as the untyped call has them.  Allowed:
+ *   fp32 solution: F in {float32, float16, bfloat16}, I in {float32, float64};
+ *   fp64 solution: F in {float64, float32},           I = float64.
+ * Every other combination is refused at the add call, naming the type and the element type.  Each narrowing is one IEEE
+ * round-to-nearest-even conversion from T: finite values beyond F's range become +-inf, subnormal results are kept (the
+ * conversions do not flush, though the engine runs fp32 arithmetic with FTZ), NaN stays NaN (payload unspecified).  Widening F
+ * to T, and T to double, is exact.  float16 and bfloat16 elements cross this ABI as their 16-bit patterns (uint16_t). */
+enum { YB_TYPE_ELEM = 0, YB_TYPE_F64 = 1, YB_TYPE_F32 = 2, YB_TYPE_F16 = 3, YB_TYPE_BF16 = 4 };
+/* yb_solution_add_slice with frames of type `frame_type`: frame[r][pt] = N_F(var(u, pt)), nrows x the owned part x sizeof(F)
+ * bytes per rank (the 64-bit byte-count refusal uses sizeof(F)); yb_solution_get_slice_frames copies out in F. */
+int yb_solution_add_slice_typed(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                int64_t t0, int64_t every, int64_t nrows, int frame_type, int64_t* id);
+/* yb_solution_add_slice_injector whose `frames` are nrows x the decimated box of type `frame_type`, widened exactly on the device:
+ *   YB_INJECT_SET: var(u, pt) = T(frame[r][pt]);   YB_INJECT_ADD: var(u, pt) = T(var(u, pt) + T(frame[r][pt])), one add in T.
+ * An injector or correlator fed from a recorder (yb_solution_add_slice_injector_from, yb_solution_add_slice_correlator with a
+ * source) reads that recorder's frame type and takes none of its own. */
+int yb_solution_add_slice_injector_typed(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                         int64_t t0, int64_t every, int64_t nrows, int mode, int frame_type, const void* frames, int64_t* id);
+/* yb_solution_add_slice_correlator with an image of type `image_type` (own_elems x sizeof(I) bytes per rank); b is read in the
+ * source recorder's frame type and widened exactly to T.  With I = T: image = T(image + T(var * b)) as the untyped call.  With
+ * I = float64 in an fp32 solution: image = image + double(var) * double(b), the product exact and the sum rounded in double
+ * (an autocorrelation: image + double(v) * double(v)).  yb_solution_get_correlator_image copies out in I. */
+int yb_solution_add_slice_correlator_typed(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                           int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse,
+                                           int image_type, int64_t* id);
+/* The frame type of recorder `id` and the image type of correlator `id`, resolved (never YB_TYPE_ELEM): the layout
+ * yb_solution_get_slice_frames and yb_solution_get_correlator_image write. */
+int yb_solution_get_slice_frame_type(yb_solution* s, int64_t id, int* type);
+int yb_solution_get_correlator_image_type(yb_solution* s, int64_t id, int* type);
+
 /* ---- multi-GPU halo exchange, one process per GPU (replaces exchange_halos, halo.cpp:80-491) --- */
 /* Each rank exports an opaque blob (CUDA IPC handles of its var storage + sync flags), the
  * launcher all-gathers the blobs (torch.distributed / MPI / files) and imports every

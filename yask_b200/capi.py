@@ -65,6 +65,8 @@ ABI_SYMBOLS = [
     "yb_solution_add_slice", "yb_solution_get_slice_frames", "yb_solution_clear_slices",
     "yb_solution_add_slice_injector", "yb_solution_clear_slice_injectors", "yb_solution_add_slice_injector_from",
     "yb_solution_add_slice_correlator", "yb_solution_get_correlator_image", "yb_solution_clear_slice_correlators",
+    "yb_solution_add_slice_typed", "yb_solution_add_slice_injector_typed", "yb_solution_add_slice_correlator_typed",
+    "yb_solution_get_slice_frame_type", "yb_solution_get_correlator_image_type",
     "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
@@ -150,6 +152,14 @@ def lib() -> C.CDLL:
                                                        i32, C.POINTER(i64)]
         L.yb_solution_get_correlator_image.argtypes = [p, i64, p, C.POINTER(C.c_uint8)]
         L.yb_solution_clear_slice_correlators.argtypes = [p]
+        L.yb_solution_add_slice_typed.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64, i32,
+                                                  C.POINTER(i64)]
+        L.yb_solution_add_slice_injector_typed.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64,
+                                                           i32, i32, p, C.POINTER(i64)]
+        L.yb_solution_add_slice_correlator_typed.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64,
+                                                             p, i64, i32, i32, C.POINTER(i64)]
+        L.yb_solution_get_slice_frame_type.argtypes = [p, i64, C.POINTER(i32)]
+        L.yb_solution_get_correlator_image_type.argtypes = [p, i64, C.POINTER(i32)]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
         L.yb_halo_export.argtypes = [p, p, C.c_size_t]
         L.yb_halo_import.argtypes = [p, i64, p, C.c_size_t]
@@ -194,6 +204,59 @@ def trilinear(pos):
     _chk(lib().yb_points_trilinear(nd, n, a.ctypes.data_as(C.POINTER(C.c_double)), idx.ctypes.data_as(C.POINTER(C.c_int64)),
                                    w.ctypes.data_as(C.POINTER(C.c_double))))
     return idx, w
+
+
+# Frame and image types of the slice calls (YB_TYPE_* of include/yask_b200.h).  numpy has no bfloat16: bf16 frames cross the
+# C ABI as uint16 bit patterns and come back widened exactly to float32.
+TYPE_ELEM, TYPE_F64, TYPE_F32, TYPE_F16, TYPE_BF16 = 0, 1, 2, 3, 4
+SLICE_TYPES = {"float64": TYPE_F64, "float32": TYPE_F32, "float16": TYPE_F16, "bfloat16": TYPE_BF16}
+
+
+def slice_type(what: str, field: str, dtype) -> int:
+    """YB_TYPE_* of a dtype argument: None (the element type), "float16", "bfloat16", "float32", "float64" or a numpy dtype."""
+    if dtype is None:
+        return TYPE_ELEM
+    if isinstance(dtype, str) and dtype in SLICE_TYPES:
+        return SLICE_TYPES[dtype]
+    try:
+        name = np.dtype(dtype).name
+    except TypeError:
+        name = None
+    if name in ("float64", "float32", "float16"):
+        return SLICE_TYPES[name]
+    raise YaskError(-1, f"{what}: unknown {field} {dtype!r} (expected 'float16', 'bfloat16', 'float32' or 'float64')")
+
+
+def bf16_bits(a) -> np.ndarray:
+    """float32 values -> bfloat16 bit patterns (uint16): IEEE round to nearest even, overflow to +-inf, subnormals kept, NaN a
+    (quiet) NaN."""
+    f = np.ascontiguousarray(a, np.float32)
+    u = f.view(np.uint32)
+    out = ((u + np.uint32(0x7FFF) + ((u >> np.uint32(16)) & np.uint32(1))) >> np.uint32(16)).astype(np.uint16)
+    nan = np.isnan(f)
+    out[nan] = ((u[nan] >> np.uint32(16)) | np.uint32(0x40)).astype(np.uint16)
+    return out
+
+
+def bf16_widen(bits) -> np.ndarray:
+    """bfloat16 bit patterns (uint16) -> float32, exactly."""
+    return (np.asarray(bits, np.uint16).astype(np.uint32) << np.uint32(16)).view(np.float32)
+
+
+def narrow_frames(a, elem_bytes: int, ftype: int) -> np.ndarray:
+    """What a host-fed injector's frames hold: the real array rounded to the element type T, then by RNE to the frame type
+    (bf16 as uint16 bit patterns)."""
+    t = np.ascontiguousarray(a, dtype=np.float32 if elem_bytes == 4 else np.float64)
+    with np.errstate(over="ignore"):
+        if ftype == TYPE_BF16:
+            return bf16_bits(t.astype(np.float32))
+        if ftype == TYPE_F16:
+            return t.astype(np.float16)
+        if ftype == TYPE_F32:
+            return t.astype(np.float32)
+        if ftype == TYPE_F64:
+            return t.astype(np.float64)
+    return t
 
 
 def _arr(vals: Sequence[int]):
@@ -516,10 +579,12 @@ class Solution:
         self._nrcv = self._nrows_r = 0
 
     # slice recorders (yb_solution_add_slice / get_slice_frames / clear_slices)
-    def add_slice(self, var: str, first, last, t0: int, nrows: int, stride=None, every: int = 1) -> int:
+    def add_slice(self, var: str, first, last, t0: int, nrows: int, stride=None, every: int = 1, dtype=None) -> int:
         """Record the box first[d], first[d] + stride[d], ... <= last[d] (global domain indices) of var(u) into frame row
         (u - t0) // every after every step u a run computes with u - t0 a multiple of `every` and the row below nrows.
-        Returns the recorder's id."""
+        dtype: the frame type ("float16", "bfloat16", "float32", "float64" or a numpy dtype; None: the element type), each
+        element rounded to it to nearest even.  Returns the recorder's id."""
+        ftype = slice_type("slice", "dtype", dtype)
         nd = len(self.get_domain_dim_names())
         f, l = np.atleast_1d(np.asarray(first, np.int64)), np.atleast_1d(np.asarray(last, np.int64))
         st = np.ones(nd, np.int64) if stride is None else np.atleast_1d(np.asarray(stride, np.int64))
@@ -528,23 +593,33 @@ class Solution:
                 raise YaskError(-1, f"slice: {what} needs {nd} domain index(es) ({', '.join(self.get_domain_dim_names())}), "
                                     f"got {a.tolist()}")
         rid = C.c_int64(-1)
-        _chk(lib().yb_solution_add_slice(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
-                                         int(t0), int(every), int(nrows), C.byref(rid)))
+        _chk(lib().yb_solution_add_slice_typed(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                               int(t0), int(every), int(nrows), ftype, C.byref(rid)))
         if not hasattr(self, "_slices"):
             self._slices = {}
         self._slices[rid.value] = (tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1), int(nrows))
         return rid.value
 
     def get_slice_frames(self, rid: int):
-        """(frames, owned): frames (nrows, *box_shape) in the element dtype, owned (box_shape) True for the points this rank
-        records; the others stay 0."""
+        """(frames, owned): frames (nrows, *box_shape) in the frame type (bfloat16 widened exactly to float32), owned
+        (box_shape) True for the points this rank records; the others stay 0."""
         shape, nrows = getattr(self, "_slices", {}).get(rid, ((0,), 0))
-        dt = np.float32 if self.get_element_bytes() == 4 else np.float64
-        out = np.zeros((nrows,) + shape, dtype=dt)
+        ftype = self._slice_type(lib().yb_solution_get_slice_frame_type, rid)
+        out = np.zeros((nrows,) + shape, dtype=self._TYPE_DTYPES[ftype])
         owned = np.zeros(shape, dtype=np.uint8)
         _chk(lib().yb_solution_get_slice_frames(self._h, int(rid), out.ctypes.data if self.is_prepared() else None,
                                                 owned.ctypes.data_as(C.POINTER(C.c_uint8))))
-        return out, owned.astype(bool)
+        return (bf16_widen(out) if ftype == TYPE_BF16 else out), owned.astype(bool)
+
+    _TYPE_DTYPES = {TYPE_F64: np.float64, TYPE_F32: np.float32, TYPE_F16: np.float16, TYPE_BF16: np.uint16}
+
+    def _slice_type(self, query, sid: int) -> int:
+        """The resolved frame or image type of recorder or correlator `sid`, or the element type when there is none (the
+        getters then refuse it themselves)."""
+        t = C.c_int(0)
+        if query(self._h, int(sid), C.byref(t)) != 0:
+            return TYPE_F32 if self.get_element_bytes() == 4 else TYPE_F64
+        return t.value
 
     def clear_slices(self):
         _chk(lib().yb_solution_clear_slices(self._h))
@@ -553,11 +628,15 @@ class Solution:
     # slice injectors (yb_solution_add_slice_injector / clear_slice_injectors)
     INJECT_MODES = {"add": 0, "set": 1}        # YB_INJECT_ADD, YB_INJECT_SET
 
-    def add_slice_injector(self, var: str, first, last, t0: int, frames, stride=None, every: int = 1, mode: str = "add") -> int:
+    def add_slice_injector(self, var: str, first, last, t0: int, frames, stride=None, every: int = 1, mode: str = "add",
+                           dtype=None) -> int:
         """After every step u a run computes with u - t0 a multiple of `every` and r = (u - t0) // every below len(frames), set
         (mode "set") or add frames[r] to (mode "add", one add in the element type) var(u) at the box first[d], first[d] +
         stride[d], ... <= last[d] (global domain indices).  frames: (nrows, *box_shape); a real array of another dtype is rounded
-        to the element type.  The frames are copied.  Returns the injector's id."""
+        to the element type.  dtype: the frame type the engine holds them in (as add_slice): the frames rounded to the element
+        type are rounded again, to nearest even, to it, and widened exactly on the device.  The frames are copied.  Returns the
+        injector's id."""
+        ftype = slice_type("slice injector", "dtype", dtype)
         nd = len(self.get_domain_dim_names())
         f, l = np.atleast_1d(np.asarray(first, np.int64)), np.atleast_1d(np.asarray(last, np.int64))
         st = np.ones(nd, np.int64) if stride is None else np.atleast_1d(np.asarray(stride, np.int64))
@@ -575,11 +654,11 @@ class Solution:
         if (l >= f).all() and (st >= 1).all() and (fr.ndim != nd + 1 or tuple(fr.shape[1:]) != box):
             raise YaskError(-1, f"slice injector: frames of shape {fr.shape} do not match the decimated box: expected "
                                 f"(nrows, {', '.join(str(b) for b in box)})")
-        fr = np.ascontiguousarray(fr, dtype=np.float32 if self.get_element_bytes() == 4 else np.float64)
+        fr = narrow_frames(fr, self.get_element_bytes(), ftype)
         rid = C.c_int64(-1)
-        _chk(lib().yb_solution_add_slice_injector(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
-                                                  int(t0), int(every), fr.shape[0] if fr.ndim else 0, self.INJECT_MODES[mode], fr.ctypes.data,
-                                                  C.byref(rid)))
+        _chk(lib().yb_solution_add_slice_injector_typed(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                        int(t0), int(every), fr.shape[0] if fr.ndim else 0, self.INJECT_MODES[mode], ftype,
+                                                        fr.ctypes.data, C.byref(rid)))
         return rid.value
 
     def clear_slice_injectors(self):
@@ -610,29 +689,30 @@ class Solution:
 
     # slice correlators (yb_solution_add_slice_correlator / get_correlator_image / clear_slice_correlators)
     def add_slice_correlator(self, var: str, first, last, t0: int, nrows: int, src: "Solution" = None, src_id: int = None,
-                             reverse: bool = False, stride=None, every: int = 1) -> int:
+                             reverse: bool = False, stride=None, every: int = 1, image_dtype=None) -> int:
         """After every step u a run computes with u - t0 a multiple of `every` and r = (u - t0) // every below nrows, add
         var(u) * b to the image at the box first[d], first[d] + stride[d], ... <= last[d], the product and the sum each rounded to
         the element type.  b is var(u) with no src (the illumination), else row r (nrows - 1 - r when reverse) of recorder src_id
-        of solution src (which may be this one).  Returns the correlator's id."""
+        of solution src (which may be this one), read in its frame type.  image_dtype "float64" in an fp32 solution holds the
+        image in double: image + double(var) * double(b), the product exact.  Returns the correlator's id."""
+        itype = slice_type("slice correlator", "image_dtype", image_dtype)
         f, l, st = self._box("slice correlator", first, last, stride)
         if src is not None and src_id is None:
             raise YaskError(-1, "slice correlator: a source solution needs src_id, the id of one of its recorders")
         rid = C.c_int64(-1)
-        _chk(lib().yb_solution_add_slice_correlator(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
-                                                    int(t0), int(every), int(nrows), None if src is None else src._h,
-                                                    0 if src_id is None else int(src_id), int(reverse), C.byref(rid)))
+        _chk(lib().yb_solution_add_slice_correlator_typed(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                          int(t0), int(every), int(nrows), None if src is None else src._h,
+                                                          0 if src_id is None else int(src_id), int(reverse), itype, C.byref(rid)))
         if not hasattr(self, "_correlators"):
             self._correlators = {}
         self._correlators[rid.value] = tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1)
         return rid.value
 
     def get_correlator_image(self, cid: int):
-        """(image, owned): image (box_shape) in the element dtype, owned (box_shape) True for the points this rank holds; the
+        """(image, owned): image (box_shape) in the image type, owned (box_shape) True for the points this rank holds; the
         others stay 0."""
         shape = getattr(self, "_correlators", {}).get(cid, (0,))
-        dt = np.float32 if self.get_element_bytes() == 4 else np.float64
-        out = np.zeros(shape, dtype=dt)
+        out = np.zeros(shape, dtype=self._TYPE_DTYPES[self._slice_type(lib().yb_solution_get_correlator_image_type, cid)])
         owned = np.zeros(shape, dtype=np.uint8)
         _chk(lib().yb_solution_get_correlator_image(self._h, int(cid), out.ctypes.data if self.is_prepared() else None,
                                                     owned.ctypes.data_as(C.POINTER(C.c_uint8))))

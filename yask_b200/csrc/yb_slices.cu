@@ -36,7 +36,65 @@ struct SliceDesc {
     // (dims right-aligned as in box), which the split form's selection tests against the interior box
     int mode;
     long long loc0[4], lstep[4];
+    int ftype, itype;               // YB_TYPE_* of the frames and (correlators) of the image; never YB_TYPE_ELEM
 };
+
+// A 16-bit frame element, held as its bit pattern.
+struct Half { unsigned short bits; };
+struct BHalf { unsigned short bits; };
+
+// N_F: IEEE round-to-nearest-even narrowing of an element to a frame type, in inline PTX without .ftz.  The engine builds with
+// -ftz=true, under which nvcc's own f64 -> f32 conversion flushes subnormal results; these keep subnormal inputs and results,
+// turn finite values beyond F's range into +-inf and keep NaN a NaN.
+template <typename F, typename T> __device__ __forceinline__ F narrow(T v) { return v; }
+template <> __device__ __forceinline__ float narrow<float, double>(double v) {
+    float o;
+    asm("cvt.rn.f32.f64 %0, %1;" : "=f"(o) : "d"(v));
+    return o;
+}
+template <> __device__ __forceinline__ Half narrow<Half, float>(float v) {
+    Half o;
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(o.bits) : "f"(v));
+    return o;
+}
+template <> __device__ __forceinline__ BHalf narrow<BHalf, float>(float v) {
+    BHalf o;
+    asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(o.bits) : "f"(v));
+    return o;
+}
+
+// Exact widening of a frame element to float or double (inline PTX for f32 -> f64: no .ftz, so subnormal inputs are kept).
+__device__ __forceinline__ float wide_f(float v) { return v; }
+__device__ __forceinline__ float wide_f(Half h) {
+    float o;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(o) : "h"(h.bits));
+    return o;
+}
+__device__ __forceinline__ float wide_f(BHalf h) { return __uint_as_float(unsigned(h.bits) << 16); }
+__device__ __forceinline__ double wide_d(double v) { return v; }
+__device__ __forceinline__ double wide_d(float v) {
+    double o;
+    asm("cvt.f64.f32 %0, %1;" : "=d"(o) : "f"(v));
+    return o;
+}
+template <typename T, typename F> __device__ __forceinline__ T widen(F v) {
+    if constexpr (sizeof(T) == 4) return wide_f(v);
+    else return wide_d(v);
+}
+
+// f(F{}) with the frame element type F that `type` names among those a solution of element type T allows (the add call refused
+// every other): fp32 solutions f32, f16, bf16; fp64 solutions f64, f32.  `type` is one descriptor's, so the branch is uniform
+// across a CTA.
+template <typename T, typename Fn> __device__ __forceinline__ void with_frame_type(int type, Fn&& f) {
+    if constexpr (sizeof(T) == 4) {
+        if (type == YB_TYPE_F16) f(Half{});
+        else if (type == YB_TYPE_BF16) f(BHalf{});
+        else f(float{});
+    } else {
+        if (type == YB_TYPE_F32) f(float{});
+        else f(double{});
+    }
+}
 
 __host__ __device__ __forceinline__ bool row_due(long long u, long long t0, long long every, long long nrows, long long& row) {
     const long long k = u - t0;
@@ -58,9 +116,12 @@ __global__ void __launch_bounds__(256) slices_kernel(const SliceDesc* __restrict
         long long slot = u % d.alloc;
         slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
         const T* __restrict__ src = reinterpret_cast<const T*>(d.var_base + slot * d.slot_bytes);
-        T* __restrict__ dst = reinterpret_cast<T*>(d.frames) + row * b.total;
-        long long coord[4];
-        for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) dst[i] = src[box_offset(b, i, coord)];
+        with_frame_type<T>(d.ftype, [&](auto tag) {
+            using F = decltype(tag);
+            F* __restrict__ dst = reinterpret_cast<F*>(d.frames) + row * b.total;
+            long long coord[4];
+            for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) dst[i] = narrow<F>(src[box_offset(b, i, coord)]);
+        });
     }
 }
 
@@ -88,28 +149,34 @@ __global__ void __launch_bounds__(256) slice_injectors_kernel(const SliceDesc* _
         long long slot = u % d.alloc;
         slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
         T* __restrict__ dst = reinterpret_cast<T*>(const_cast<char*>(d.var_base) + slot * d.slot_bytes);
-        const T* __restrict__ src = reinterpret_cast<const T*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total;
         const bool set = d.mode == YB_INJECT_SET;
-        long long coord[4];
-        for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) {
-            const long long o = box_offset(b, i, coord);
-            if (q.sel != PTS_ALL) {
-                bool in = true;
+        with_frame_type<T>(d.ftype, [&](auto tag) {
+            using F = decltype(tag);
+            const F* __restrict__ src = reinterpret_cast<const F*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total;
+            long long coord[4];
+            for (long long i = blockIdx.x * 256ll + threadIdx.x; i < b.total; i += gridDim.x * 256ll) {
+                const long long o = box_offset(b, i, coord);
+                if (q.sel != PTS_ALL) {
+                    bool in = true;
 #pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    const long long c = d.loc0[k] + coord[k] * d.lstep[k];
-                    in = in && c >= q.ib[k] && c < q.ie[k];
+                    for (int k = 0; k < 4; k++) {
+                        const long long c = d.loc0[k] + coord[k] * d.lstep[k];
+                        in = in && c >= q.ib[k] && c < q.ie[k];
+                    }
+                    if (in != (q.sel == PTS_INTERIOR)) continue;
                 }
-                if (in != (q.sel == PTS_INTERIOR)) continue;
+                const T f = widen<T>(src[i]);
+                dst[o] = set ? f : add_elem(dst[o], f);
             }
-            dst[o] = set ? src[i] : add_elem(dst[o], src[i]);
-        }
+        });
     }
 }
 
 // the imaging condition's rounding: the product and the sum each rounded, never fused
 __device__ __forceinline__ float mul_add_rn(float img, float v, float b) { return __fadd_rn(img, __fmul_rn(v, b)); }
 __device__ __forceinline__ double mul_add_rn(double img, double v, double b) { return __dadd_rn(img, __dmul_rn(v, b)); }
+// a double image of an fp32 solution: img + double(v) * double(b), the product exact and the sum rounded
+__device__ __forceinline__ double mul_add_rn(double img, float v, float b) { return __dadd_rn(img, __dmul_rn(wide_d(v), wide_d(b))); }
 
 // blockIdx.y walks the correlators (each writes only its own image, so all the due ones share a launch).  blockIdx.x and the
 // threads walk rows of the unit-stride dim, 2^lanes_log2 threads per row: a row's storage offset is computed once, with the two
@@ -127,25 +194,35 @@ __global__ void __launch_bounds__(256) slice_correlators_kernel(const SliceDesc*
         long long slot = u % d.alloc;
         slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
         const T* __restrict__ var = reinterpret_cast<const T*>(d.var_base + slot * d.slot_bytes) + b.off;
-        const T* __restrict__ src = d.frames ? reinterpret_cast<const T*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total : nullptr;
-        T* __restrict__ img = reinterpret_cast<T*>(d.image);
         const int lg = d.lanes_log2, lanes = 1 << lg;
         const long long len = b.n[3], vs = b.vs[3], rows = b.n[0] * b.n[1] * b.n[2], per = 256 >> lg;
         const int lane = threadIdx.x & (lanes - 1);
-        for (long long q = blockIdx.x * per + (threadIdx.x >> lg); q < rows; q += gridDim.x * per) {
-            const long long q1 = q / b.n[2], c2 = q - q1 * b.n[2];
-            const long long c0 = q1 / b.n[1], c1 = q1 - c0 * b.n[1];
-            const T* __restrict__ vrow = var + c0 * b.vs[0] + c1 * b.vs[1] + c2 * b.vs[2];
-            const long long o = q * len;
-            if (src) {
-                for (long long i = lane; i < len; i += lanes) img[o + i] = mul_add_rn(img[o + i], vrow[i * vs], src[o + i]);
-            } else {
-                for (long long i = lane; i < len; i += lanes) {
-                    const T v = vrow[i * vs];
-                    img[o + i] = mul_add_rn(img[o + i], v, v);
+        // the frame type F (an autocorrelation has no frames: its descriptor names T) and the image type I: T or, in an fp32
+        // solution, double
+        with_frame_type<T>(d.ftype, [&](auto ftag) {
+            using F = decltype(ftag);
+            const F* __restrict__ src = d.frames ? reinterpret_cast<const F*>(d.frames) + (d.rev ? d.nrows - 1 - row : row) * b.total : nullptr;
+            auto walk = [&](auto itag) {
+                using I = decltype(itag);
+                I* __restrict__ img = reinterpret_cast<I*>(d.image);
+                for (long long q = blockIdx.x * per + (threadIdx.x >> lg); q < rows; q += gridDim.x * per) {
+                    const long long q1 = q / b.n[2], c2 = q - q1 * b.n[2];
+                    const long long c0 = q1 / b.n[1], c1 = q1 - c0 * b.n[1];
+                    const T* __restrict__ vrow = var + c0 * b.vs[0] + c1 * b.vs[1] + c2 * b.vs[2];
+                    const long long o = q * len;
+                    if (src) {
+                        for (long long i = lane; i < len; i += lanes) img[o + i] = mul_add_rn(img[o + i], vrow[i * vs], widen<T>(src[o + i]));
+                    } else {
+                        for (long long i = lane; i < len; i += lanes) {
+                            const T v = vrow[i * vs];
+                            img[o + i] = mul_add_rn(img[o + i], v, v);
+                        }
+                    }
                 }
-            }
-        }
+            };
+            if (sizeof(T) == 4 && d.itype == YB_TYPE_F64) walk(double{});
+            else walk(T{});
+        });
     }
 }
 
@@ -258,6 +335,36 @@ int plan_one(const Solution& s, const SlicesState& p, SliceRec& r) {
 // rank-local coordinate of the first owned point in domain dim k (the last one is that + (own_n[k] - 1) * stride[k])
 int64_t own_loc0(const Solution& s, const SliceRec& r, int k) { return r.first[k] + r.own_k0[k] * r.stride[k] - s.rank_offset[k]; }
 
+int elem_type(const Solution& s) { return s.spec.elem_bytes == 4 ? YB_TYPE_F32 : YB_TYPE_F64; }
+
+int type_bytes(int type) { return type == YB_TYPE_F64 ? 8 : type == YB_TYPE_F32 ? 4 : 2; }
+
+const char* type_name(int type) {
+    return type == YB_TYPE_F64 ? "float64" : type == YB_TYPE_F32 ? "float32" : type == YB_TYPE_F16 ? "float16" : "bfloat16";
+}
+
+// The frame type (image = false) or image type of a new recorder, injector or correlator: YB_TYPE_ELEM is the element type;
+// otherwise refused unless the table of include/yask_b200.h allows it in this solution.
+int resolve_type(const Solution& s, const char* what, int type, bool image, int& out) {
+    const int et = elem_type(s);
+    const char* field = image ? "image" : "frame";
+    if (type == YB_TYPE_ELEM) {
+        out = et;
+        return 0;
+    }
+    if (type < YB_TYPE_F64 || type > YB_TYPE_BF16)
+        return set_error(YB_EINVAL, "%s: unknown %s type %d (YB_TYPE_ELEM, YB_TYPE_F64, YB_TYPE_F32, YB_TYPE_F16 or YB_TYPE_BF16)", what,
+                         field, type);
+    const bool ok = image ? type == YB_TYPE_F64 || type == et : et == YB_TYPE_F32 ? type != YB_TYPE_F64 : type == YB_TYPE_F64 || type == YB_TYPE_F32;
+    if (!ok)
+        return set_error(YB_EINVAL, "%s: %s type %s is not allowed in a solution of element type %s (allowed: %s)", what, field,
+                         type_name(type), type_name(et),
+                         image ? (et == YB_TYPE_F32 ? "float32, float64" : "float64")
+                               : (et == YB_TYPE_F32 ? "float32, float16, bfloat16" : "float64, float32"));
+    out = type;
+    return 0;
+}
+
 // a correlator's threads per row of the unit-stride dim of `len` points: the power of two at or above it, up to the CTA's 256
 int lanes_log2(int64_t len) {
     int lg = 0;
@@ -289,6 +396,8 @@ SliceDesc describe(const Solution& s, const SliceRec& r) {
     d.image = static_cast<char*>(r.image.get());
     d.rev = r.rev;
     d.lanes_log2 = lanes_log2(d.box.n[3]);
+    d.ftype = r.ftype;
+    d.itype = r.itype;
     return d;
 }
 
@@ -312,7 +421,8 @@ int alloc_frames(const Solution& s, const SlicesState& p, SliceRec& r) {
     const bool corr = p.kind == SLICE_CORRELATE;
     std::shared_ptr<void>& buf = corr ? r.image : r.frames;
     const int64_t rows = corr ? 1 : r.nrows;
-    const size_t bytes = size_t(rows) * size_t(r.own_elems) * s.spec.elem_bytes;
+    const size_t eb = size_t(type_bytes(corr ? r.itype : r.ftype));
+    const size_t bytes = size_t(rows) * size_t(r.own_elems) * eb;
     if (buf || (r.link && !corr)) return 0;
     if (!bytes) {
         std::vector<char>().swap(r.host_frames);
@@ -334,7 +444,6 @@ int alloc_frames(const Solution& s, const SlicesState& p, SliceRec& r) {
         YB_CUDA(cudaMemset(d, 0, bytes));
         return 0;
     }
-    const size_t eb = size_t(s.spec.elem_bytes);
     std::vector<char> dense(bytes);
     owned_runs(s, r, r.nrows, [&](size_t whole, size_t own, size_t n) { memcpy(dense.data() + own * eb, r.host_frames.data() + whole * eb, n * eb); });
     YB_CUDA(cudaMemcpy(d, dense.data(), bytes, cudaMemcpyHostToDevice));
@@ -605,9 +714,12 @@ using namespace yb;
 // The checks shared by recorders and injectors: the var, the box, the window and a 64-bit byte count of the frames of the whole
 // box (which bound every rank's share).  Fills r up to the window; `bytes`: nrows x the decimated box in bytes.
 static int new_rec(Solution* s, const char* what, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
-                   int64_t t0, int64_t every, int64_t nrows, SliceRec& r, int64_t& bytes) {
+                   int64_t t0, int64_t every, int64_t nrows, int frame_type, SliceRec& r, int64_t& bytes) {
     if (!first || !last) return set_error(YB_EINVAL, "%s: null box", what);
     if (int rc = point_var(*s, what, var, r.var, r.step_off)) return rc;
+    if (int rc = resolve_type(*s, what, frame_type, false, r.ftype)) return rc;
+    r.itype = elem_type(*s);
+    const int fb = type_bytes(r.ftype);
     for (int k = 0; k < s->ndd; k++) {
         const char* dn = s->spec.domain_dims[k].c_str();
         r.first[k] = first[k];
@@ -623,11 +735,10 @@ static int new_rec(Solution* s, const char* what, const char* var, const int64_t
     int64_t points = 1;
     bool over = false;
     for (int k = 0; k < s->ndd; k++) over = over || __builtin_mul_overflow(points, r.count[k], &points);
-    over = over || __builtin_mul_overflow(points, nrows, &bytes) || __builtin_mul_overflow(bytes, int64_t(s->spec.elem_bytes), &bytes);
+    over = over || __builtin_mul_overflow(points, nrows, &bytes) || __builtin_mul_overflow(bytes, int64_t(fb), &bytes);
     if (over)
         return set_error(YB_ERANGE, "%s: %lld rows of the decimated box (%lld x %lld x %lld points) of %d-byte elements overflow a 64-bit "
-                         "byte count", what, (long long)nrows, (long long)r.count[0], (long long)r.count[1], (long long)r.count[2],
-                         s->spec.elem_bytes);
+                         "byte count", what, (long long)nrows, (long long)r.count[0], (long long)r.count[1], (long long)r.count[2], fb);
     r.t0 = t0; r.every = every; r.nrows = nrows;
     return 0;
 }
@@ -685,6 +796,7 @@ static int attach(Solution* s, SlicesState*& pp, SliceKind kind, SliceRec& r, yb
     auto link = std::make_shared<FrameLink>();
     link->device = src->device;
     link->elem_bytes = src->spec.elem_bytes;
+    link->ftype = q.ftype;
     link->ndd = src->ndd;
     link->src_id = src_id;
     link->nrows = q.nrows;
@@ -694,6 +806,7 @@ static int attach(Solution* s, SlicesState*& pp, SliceKind kind, SliceRec& r, yb
         link->own_k0[k] = q.own_k0[k]; link->own_n[k] = q.own_n[k];
     }
     r.link = link;
+    r.ftype = link->ftype;
     if (int rc = check_mode(*s, p)) return rc;
     if (int rc = plan_one(*s, p, r)) return rc;
     if (!src->prepared)
@@ -726,7 +839,7 @@ static int clear_state(Solution* s, SlicesState*& p, SliceKind kind) {
 
 // `rows` rows of the whole decimated box of r into out from `dev` (rows x this rank's part; null when nothing was allocated), 0
 // where this rank owns no point, and the owned mask.  `out` may be null: the mask only, which needs no device.
-static int copy_out(Solution* s, const SliceRec& r, const void* dev, int64_t rows, void* out, uint8_t* owned) {
+static int copy_out(Solution* s, const SliceRec& r, const void* dev, int64_t rows, int type, void* out, uint8_t* owned) {
     size_t box = 1;
     for (int k = 0; k < s->ndd; k++) box *= size_t(r.count[k]);
     if (owned) {
@@ -734,7 +847,7 @@ static int copy_out(Solution* s, const SliceRec& r, const void* dev, int64_t row
         owned_runs(*s, r, 1, [&](size_t whole, size_t, size_t n) { memset(owned + whole, 1, n); });
     }
     if (!out) return 0;
-    const size_t eb = size_t(s->spec.elem_bytes);
+    const size_t eb = size_t(type_bytes(type));
     memset(out, 0, size_t(rows) * box * eb);
     if (!dev) return 0;
     std::vector<char> dense(size_t(rows) * size_t(r.own_elems) * eb);
@@ -747,24 +860,29 @@ static int copy_out(Solution* s, const SliceRec& r, const void* dev, int64_t row
 
 extern "C" {
 
-int yb_solution_add_slice(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
-                          int64_t t0, int64_t every, int64_t nrows, int64_t* id) {
+int yb_solution_add_slice_typed(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                int64_t t0, int64_t every, int64_t nrows, int frame_type, int64_t* id) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
     SliceRec r;
     int64_t bytes = 0;
-    if (int rc = new_rec(s, "slice", var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (int rc = new_rec(s, "slice", var, first, last, stride, t0, every, nrows, frame_type, r, bytes)) return rc;
     return install(s, s->slices, SLICE_RECORD, std::move(r), id);
 }
 
-int yb_solution_add_slice_injector(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
-                                   int64_t t0, int64_t every, int64_t nrows, int mode, const void* frames, int64_t* id) {
+int yb_solution_add_slice(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                          int64_t t0, int64_t every, int64_t nrows, int64_t* id) {
+    return yb_solution_add_slice_typed(s, var, first, last, stride, t0, every, nrows, YB_TYPE_ELEM, id);
+}
+
+int yb_solution_add_slice_injector_typed(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                         int64_t t0, int64_t every, int64_t nrows, int mode, int frame_type, const void* frames, int64_t* id) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
     const char* what = "slice injector";
     SliceRec r;
     int64_t bytes = 0;
-    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, frame_type, r, bytes)) return rc;
     if (mode != YB_INJECT_ADD && mode != YB_INJECT_SET)
         return set_error(YB_EINVAL, "%s: unknown mode %d (YB_INJECT_ADD = %d or YB_INJECT_SET = %d)", what, mode, YB_INJECT_ADD, YB_INJECT_SET);
     if (!frames) return set_error(YB_EINVAL, "%s: null frames", what);
@@ -777,6 +895,11 @@ int yb_solution_add_slice_injector(yb_solution* s_, const char* var, const int64
     return install(s, s->injectors, SLICE_INJECT, std::move(r), id);
 }
 
+int yb_solution_add_slice_injector(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                   int64_t t0, int64_t every, int64_t nrows, int mode, const void* frames, int64_t* id) {
+    return yb_solution_add_slice_injector_typed(s, var, first, last, stride, t0, every, nrows, mode, YB_TYPE_ELEM, frames, id);
+}
+
 int yb_solution_add_slice_injector_from(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
                                         int64_t t0, int64_t every, int64_t nrows, int mode, yb_solution* src, int64_t src_id, int reverse,
                                         int64_t* id) {
@@ -785,7 +908,7 @@ int yb_solution_add_slice_injector_from(yb_solution* s_, const char* var, const 
     const char* what = "slice injector";
     SliceRec r;
     int64_t bytes = 0;
-    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, YB_TYPE_ELEM, r, bytes)) return rc;
     if (mode != YB_INJECT_ADD && mode != YB_INJECT_SET)
         return set_error(YB_EINVAL, "%s: unknown mode %d (YB_INJECT_ADD = %d or YB_INJECT_SET = %d)", what, mode, YB_INJECT_ADD, YB_INJECT_SET);
     r.mode = mode;
@@ -793,19 +916,45 @@ int yb_solution_add_slice_injector_from(yb_solution* s_, const char* var, const 
     return install(s, s->injectors, SLICE_INJECT, std::move(r), id);
 }
 
-int yb_solution_add_slice_correlator(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
-                                     int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id) {
+int yb_solution_add_slice_correlator_typed(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                           int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse,
+                                           int image_type, int64_t* id) {
     Solution* s = SOL(s_);
     if (!s) return set_error(YB_EINVAL, "null solution");
+    const char* what = "slice correlator";
     SliceRec r;
     int64_t bytes = 0;
-    if (int rc = new_rec(s, "slice correlator", var, first, last, stride, t0, every, nrows, r, bytes)) return rc;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, YB_TYPE_ELEM, r, bytes)) return rc;
+    if (int rc = resolve_type(*s, what, image_type, true, r.itype)) return rc;
     if (src) {
         if (int rc = attach(s, s->correlators, SLICE_CORRELATE, r, src, src_id, reverse)) return rc;
     } else if (reverse != 0 && reverse != 1) {
         return set_error(YB_EINVAL, "slice correlator: reverse = %d is not 0 or 1", reverse);
     }
     return install(s, s->correlators, SLICE_CORRELATE, std::move(r), id);
+}
+
+int yb_solution_add_slice_correlator(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                     int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id) {
+    return yb_solution_add_slice_correlator_typed(s, var, first, last, stride, t0, every, nrows, src, src_id, reverse, YB_TYPE_ELEM, id);
+}
+
+int yb_solution_get_slice_frame_type(yb_solution* s_, int64_t id, int* type) {
+    Solution* s = SOL(s_);
+    if (!s || !type) return set_error(YB_EINVAL, "null solution or type");
+    if (!slices_active(*s) || id < 0 || id >= int64_t(s->slices->recs.size()))
+        return set_error(YB_EINVAL, "get_slice_frame_type: no slice recorder %lld", (long long)id);
+    *type = s->slices->recs[size_t(id)].ftype;
+    return 0;
+}
+
+int yb_solution_get_correlator_image_type(yb_solution* s_, int64_t id, int* type) {
+    Solution* s = SOL(s_);
+    if (!s || !type) return set_error(YB_EINVAL, "null solution or type");
+    if (!slice_correlators_active(*s) || id < 0 || id >= int64_t(s->correlators->recs.size()))
+        return set_error(YB_EINVAL, "get_correlator_image_type: no slice correlator %lld", (long long)id);
+    *type = s->correlators->recs[size_t(id)].itype;
+    return 0;
 }
 
 int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t* owned) {
@@ -817,7 +966,7 @@ int yb_solution_get_slice_frames(yb_solution* s_, int64_t id, void* out, uint8_t
     SliceRec& r = s->slices->recs[size_t(id)];
     if (!s->prepared)
         if (int rc = plan_one(*s, *s->slices, r)) return rc;
-    return copy_out(s, r, r.frames.get(), r.nrows, out, owned);
+    return copy_out(s, r, r.frames.get(), r.nrows, r.ftype, out, owned);
 }
 
 int yb_solution_get_correlator_image(yb_solution* s_, int64_t id, void* out, uint8_t* owned) {
@@ -829,7 +978,7 @@ int yb_solution_get_correlator_image(yb_solution* s_, int64_t id, void* out, uin
     SliceRec& r = s->correlators->recs[size_t(id)];
     if (!s->prepared)
         if (int rc = plan_one(*s, *s->correlators, r)) return rc;
-    return copy_out(s, r, r.image.get(), 1, out, owned);
+    return copy_out(s, r, r.image.get(), 1, r.itype, out, owned);
 }
 
 int yb_solution_clear_slices(yb_solution* s_) {

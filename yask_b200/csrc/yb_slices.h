@@ -27,6 +27,7 @@ namespace yb {
 // consumer itself.  Held by the consumer; the source keeps a weak reference (SlicesState::readers).
 struct FrameLink {
     int device = -1, elem_bytes = 0, ndd = 0;
+    int ftype = 0;                              // the recorder's frame type (YB_TYPE_*), which the consumer reads
     int64_t src_id = 0, nrows = 0;
     int64_t first[3] = {0, 0, 0}, last[3] = {0, 0, 0}, stride[3] = {1, 1, 1};
     int64_t overall[3] = {0, 0, 0}, num_ranks[3] = {1, 1, 1}, rank_index[3] = {0, 0, 0};
@@ -46,9 +47,10 @@ struct SliceRec {
     int64_t own_k0[3] = {0, 0, 0}, own_n[3] = {0, 0, 0};
     int64_t own_off = 0;                        // element offset of its first point in a step slot of the var
     int64_t own_elems = 0;
-    // nrows x own_elems elements of the solution's type: a recorder's frames, the frames an injector reads (its own, or a
+    // nrows x own_elems elements of the frame type: a recorder's frames, the frames an injector reads (its own, or a
     // recorder's), a correlator's source frames (null: autocorrelation).  Freed with cudaFree by the last holder.
     std::shared_ptr<void> frames;
+    int ftype = 0;                              // YB_TYPE_* of the frames, resolved (a consumer of a recorder: the recorder's)
     // the var's storage and slot_bias as the device table holds them (fuse_vars and the offline tuner's pairs move them)
     const void* uploaded_base = nullptr;
     int uploaded_bias = -1;
@@ -59,7 +61,8 @@ struct SliceRec {
     int rev = 0;                                // row r reads frame row nrows - 1 - r
     std::shared_ptr<FrameLink> link;
     // correlators only
-    std::shared_ptr<void> image;                // own_elems elements, zeroed at allocation
+    std::shared_ptr<void> image;                // own_elems elements of the image type, zeroed at allocation
+    int itype = 0;                              // YB_TYPE_* of the image, resolved
 };
 
 enum SliceKind { SLICE_RECORD, SLICE_INJECT, SLICE_CORRELATE };

@@ -958,15 +958,92 @@ B200Solution& b200_slices(const yk_solution_ptr& soln) {
 }
 }  // namespace
 
+namespace {
+// YB_TYPE_* of a frame or image type name ("" is the element type)
+int slice_type(const char* what, const char* field, const std::string& name) {
+    if (name.empty()) return YB_TYPE_ELEM;
+    if (name == "float64") return YB_TYPE_F64;
+    if (name == "float32") return YB_TYPE_F32;
+    if (name == "float16") return YB_TYPE_F16;
+    if (name == "bfloat16") return YB_TYPE_BF16;
+    fail(std::string(what) + ": unknown " + field + " '" + name + "' (expected float16, bfloat16, float32 or float64)");
+    return YB_TYPE_ELEM;
+}
+
+int type_bytes(int type) { return type == YB_TYPE_F64 ? 8 : type == YB_TYPE_F32 ? 4 : 2; }
+
+// float -> IEEE half bits, round to nearest even: overflow to +-inf, subnormal results kept, NaN a quiet NaN
+uint16_t half_bits(float v) {
+    uint32_t f;
+    memcpy(&f, &v, 4);
+    const uint32_t sign = f & 0x80000000u;
+    f ^= sign;
+    uint16_t o;
+    if (f >= (127u + 16u) << 23) {                      // |v| >= 2^16 (inf, NaN)
+        o = f > 255u << 23 ? 0x7e00 : 0x7c00;
+    } else if (f < 113u << 23) {                        // |v| < 2^-14: a half subnormal or zero; adding 0.5f rounds to its grid
+        const uint32_t magic = 126u << 23;
+        float x, m;
+        memcpy(&x, &f, 4);
+        memcpy(&m, &magic, 4);
+        x += m;
+        uint32_t xi;
+        memcpy(&xi, &x, 4);
+        o = uint16_t(xi - magic);
+    } else {                                            // normal: rebias, round the 13 dropped bits to nearest even
+        f += (uint32_t(15 - 127) << 23) + 0xfffu + ((f >> 13) & 1u);
+        o = uint16_t(f >> 13);                          // a carry past 65504 gives 0x7c00, inf
+    }
+    return uint16_t(o | (sign >> 16));
+}
+
+double half_value(uint16_t h) {
+    const int e = (h >> 10) & 0x1f, m = h & 0x3ff;
+    const double v = e == 0 ? std::ldexp(double(m), -24) : e == 31 ? (m ? NAN : INFINITY) : std::ldexp(double(m | 0x400), e - 25);
+    return h & 0x8000 ? -v : v;
+}
+
+// float -> bfloat16 bits, round to nearest even (NaN a quiet NaN)
+uint16_t bf16_bits(float v) {
+    uint32_t f;
+    memcpy(&f, &v, 4);
+    if (std::isnan(v)) return uint16_t((f >> 16) | 0x40);
+    return uint16_t((f + 0x7fffu + ((f >> 16) & 1u)) >> 16);
+}
+
+double bf16_value(uint16_t b) {
+    const uint32_t f = uint32_t(b) << 16;
+    float v;
+    memcpy(&v, &f, 4);
+    return v;
+}
+
+// element i of a buffer of YB_TYPE_* `type`, widened exactly to double
+double widened(const std::vector<char>& raw, int type, size_t i) {
+    const char* p = raw.data() + i * size_t(type_bytes(type));
+    if (type == YB_TYPE_F64) { double v; memcpy(&v, p, 8); return v; }
+    if (type == YB_TYPE_F32) { float v; memcpy(&v, p, 4); return v; }
+    uint16_t h;
+    memcpy(&h, p, 2);
+    return type == YB_TYPE_F16 ? half_value(h) : bf16_value(h);
+}
+}  // namespace
+
 idx_t yk_add_slice(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0, idx_t nrows,
                    const idx_t_vec& stride, idx_t every) {
+    return yk_add_slice_typed(soln, var, first, last, t0, nrows, "", stride, every);
+}
+
+idx_t yk_add_slice_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0, idx_t nrows,
+                         const std::string& dtype, const idx_t_vec& stride, idx_t every) {
     B200Solution& s = b200_slices(soln);
     const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
     if (first.size() != nd || last.size() != nd || (!stride.empty() && stride.size() != nd))
         fail("slice: first, last and stride need " + std::to_string(nd) + " domain indices each");
+    const int type = slice_type("slice", "dtype", dtype);
     const std::vector<int64_t> f(first.begin(), first.end()), l(last.begin(), last.end()), st(stride.begin(), stride.end());
     int64_t id = -1;
-    chk(yb_solution_add_slice(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, &id));
+    chk(yb_solution_add_slice_typed(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, type, &id));
     idx_t_vec shape{nrows};
     for (size_t k = 0; k < nd; k++) shape.push_back((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1);
     s.slice_shape.resize(size_t(id) + 1);
@@ -981,13 +1058,13 @@ void yk_get_slice_frames(yk_solution_ptr soln, idx_t id, std::vector<double>& fr
     size_t box = 1;
     for (size_t k = 1; k < shape.size(); k++) box *= size_t(shape[k]);
     const size_t n = size_t(shape[0]) * box;
-    const int eb = yb_solution_elem_bytes(s.h->s);
-    std::vector<char> raw(n * eb);
+    int type = 0;
+    chk(yb_solution_get_slice_frame_type(s.h->s, id, &type));
+    std::vector<char> raw(n * size_t(type_bytes(type)));
     std::vector<uint8_t> own(box);
     chk(yb_solution_get_slice_frames(s.h->s, id, yb_solution_is_prepared(s.h->s) ? raw.data() : nullptr, own.data()));
     frames.resize(n);
-    for (size_t i = 0; i < n; i++)
-        frames[i] = eb == 4 ? double(reinterpret_cast<const float*>(raw.data())[i]) : reinterpret_cast<const double*>(raw.data())[i];
+    for (size_t i = 0; i < n; i++) frames[i] = widened(raw, type, i);
     owned.assign(own.begin(), own.end());
 }
 
@@ -1005,7 +1082,14 @@ idx_t yk_get_slice_launches(yk_solution_ptr soln) {
 
 idx_t yk_add_slice_injector(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
                             idx_t nrows, const std::vector<double>& frames, const idx_t_vec& stride, idx_t every, bool set) {
+    return yk_add_slice_injector_typed(soln, var, first, last, t0, nrows, frames, "", stride, every, set);
+}
+
+idx_t yk_add_slice_injector_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                  idx_t nrows, const std::vector<double>& frames, const std::string& dtype, const idx_t_vec& stride,
+                                  idx_t every, bool set) {
     B200Solution& s = b200_slices(soln);
+    int type = slice_type("slice injector", "dtype", dtype);
     const size_t nd = size_t(yb_solution_num_domain_dims(s.h->s));
     if (first.size() != nd || last.size() != nd || (!stride.empty() && stride.size() != nd))
         fail("slice injector: first, last and stride need " + std::to_string(nd) + " domain indices each");
@@ -1016,14 +1100,21 @@ idx_t yk_add_slice_injector(yk_solution_ptr soln, const std::string& var, const 
         fail("slice injector: " + std::to_string(frames.size()) + " frame values given, nrows x the decimated box is " + std::to_string(n));
     int64_t id = -1;
     const int mode = set ? YB_INJECT_SET : YB_INJECT_ADD;
-    if (yb_solution_elem_bytes(s.h->s) == 4) {
-        const std::vector<float> fr(frames.begin(), frames.end());       // rounded once to the element type
-        chk(yb_solution_add_slice_injector(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, mode,
-                                           fr.data(), &id));
-    } else {
-        chk(yb_solution_add_slice_injector(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, mode,
-                                           frames.data(), &id));
+    const bool f32 = yb_solution_elem_bytes(s.h->s) == 4;
+    if (type == YB_TYPE_ELEM) type = f32 ? YB_TYPE_F32 : YB_TYPE_F64;
+    // each value rounded to the element type, then to the frame type (a type the solution does not allow is refused below)
+    std::vector<char> fr(frames.size() * size_t(type_bytes(type)));
+    for (size_t i = 0; i < frames.size(); i++) {
+        const double t = f32 ? double(float(frames[i])) : frames[i];
+        char* p = fr.data() + i * size_t(type_bytes(type));
+        if (type == YB_TYPE_F64) { memcpy(p, &t, 8); continue; }
+        const float v = float(t);
+        if (type == YB_TYPE_F32) { memcpy(p, &v, 4); continue; }
+        const uint16_t h = type == YB_TYPE_F16 ? half_bits(v) : bf16_bits(v);
+        memcpy(p, &h, 2);
     }
+    chk(yb_solution_add_slice_injector_typed(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows, mode,
+                                             type, fr.data(), &id));
     return idx_t(id);
 }
 
@@ -1061,12 +1152,19 @@ idx_t yk_add_slice_injector_from(yk_solution_ptr soln, const std::string& var, c
 
 idx_t yk_add_slice_correlator(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
                               idx_t nrows, yk_solution_ptr src, idx_t src_id, bool reverse, const idx_t_vec& stride, idx_t every) {
+    return yk_add_slice_correlator_typed(soln, var, first, last, t0, nrows, "", src, src_id, reverse, stride, every);
+}
+
+idx_t yk_add_slice_correlator_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                    idx_t nrows, const std::string& image_dtype, yk_solution_ptr src, idx_t src_id, bool reverse,
+                                    const idx_t_vec& stride, idx_t every) {
     B200Solution& s = b200_slices(soln);
     std::vector<int64_t> f, l, st;
     slice_box(s, "slice correlator", first, last, stride, f, l, st);
+    const int type = slice_type("slice correlator", "image_dtype", image_dtype);
     int64_t id = -1;
-    chk(yb_solution_add_slice_correlator(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows,
-                                         src ? b200_slices(src).h->s : nullptr, src_id, reverse ? 1 : 0, &id));
+    chk(yb_solution_add_slice_correlator_typed(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows,
+                                               src ? b200_slices(src).h->s : nullptr, src_id, reverse ? 1 : 0, type, &id));
     idx_t_vec shape;
     for (size_t k = 0; k < f.size(); k++) shape.push_back((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1);
     s.correlator_shape.resize(size_t(id) + 1);
@@ -1080,13 +1178,13 @@ void yk_get_correlator_image(yk_solution_ptr soln, idx_t id, std::vector<double>
     shape = s.correlator_shape[size_t(id)];
     size_t n = 1;
     for (idx_t e : shape) n *= size_t(e);
-    const int eb = yb_solution_elem_bytes(s.h->s);
-    std::vector<char> raw(n * eb);
+    int type = 0;
+    chk(yb_solution_get_correlator_image_type(s.h->s, id, &type));
+    std::vector<char> raw(n * size_t(type_bytes(type)));
     std::vector<uint8_t> own(n);
     chk(yb_solution_get_correlator_image(s.h->s, id, yb_solution_is_prepared(s.h->s) ? raw.data() : nullptr, own.data()));
     image.resize(n);
-    for (size_t i = 0; i < n; i++)
-        image[i] = eb == 4 ? double(reinterpret_cast<const float*>(raw.data())[i]) : reinterpret_cast<const double*>(raw.data())[i];
+    for (size_t i = 0; i < n; i++) image[i] = widened(raw, type, i);
     owned.assign(own.begin(), own.end());
 }
 

@@ -338,4 +338,13 @@ PYBIND11_MODULE(yask_kernel, m) {
     }, py::arg("soln"), py::arg("id"), "(image as a flat list of floats, shape (box extents...), owned per box point)");
     m.def("yk_clear_slice_correlators", &yk_clear_slice_correlators, py::arg("soln"));
     m.def("yk_get_slice_correlator_launches", &yk_get_slice_correlator_launches, py::arg("soln"));
+    // ---- frame and image types of the slice calls ("float16", "bfloat16", "float32", "float64"; "" the element type) ----
+    m.def("yk_add_slice_typed", &yk_add_slice_typed, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"), py::arg("t0"),
+          py::arg("nrows"), py::arg("dtype"), py::arg("stride") = idx_t_vec{}, py::arg("every") = 1);
+    m.def("yk_add_slice_injector_typed", &yk_add_slice_injector_typed, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
+          py::arg("t0"), py::arg("nrows"), py::arg("frames"), py::arg("dtype"), py::arg("stride") = idx_t_vec{}, py::arg("every") = 1,
+          py::arg("set") = false);
+    m.def("yk_add_slice_correlator_typed", &yk_add_slice_correlator_typed, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
+          py::arg("t0"), py::arg("nrows"), py::arg("image_dtype"), py::arg("src") = yk_solution_ptr(), py::arg("src_id") = 0,
+          py::arg("reverse") = false, py::arg("stride") = idx_t_vec{}, py::arg("every") = 1);
 }

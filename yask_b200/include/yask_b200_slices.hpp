@@ -70,4 +70,20 @@ void yk_clear_slice_correlators(yk_solution_ptr soln);
 // Correlating launches since prepare_solution().
 idx_t yk_get_slice_correlator_launches(yk_solution_ptr soln);
 
+// Frame and image types (the typed calls): "float16", "bfloat16", "float32" or "float64"; "" is the element type.  Allowed
+// combinations, rounding and storage: YB_TYPE_* and the typed calls in include/yask_b200.h.  The getters above widen every type
+// to double exactly.
+//
+// A recorder whose frames are held in `dtype`: frame[r][pt] = var(u, pt) rounded to nearest even.
+idx_t yk_add_slice_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0, idx_t nrows,
+                         const std::string& dtype, const idx_t_vec& stride = {}, idx_t every = 1);
+// A host-fed injector whose frames are held in `dtype`: each value is rounded to the element type, then to nearest even to dtype.
+idx_t yk_add_slice_injector_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                  idx_t nrows, const std::vector<double>& frames, const std::string& dtype, const idx_t_vec& stride = {},
+                                  idx_t every = 1, bool set = false);
+// A correlator whose image is held in `image_dtype` ("float64" in an fp32 solution: image + double(var) * double(b)).
+idx_t yk_add_slice_correlator_typed(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                    idx_t nrows, const std::string& image_dtype, yk_solution_ptr src = nullptr, idx_t src_id = 0,
+                                    bool reverse = false, const idx_t_vec& stride = {}, idx_t every = 1);
+
 }  // namespace yask
