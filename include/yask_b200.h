@@ -333,13 +333,35 @@ int yb_solution_add_slice_injector_from(yb_solution* s, const char* var, const i
  * prepared solution (which synchronizes its stream), otherwise at prepare -- never in run_solution().  While any correlator is
  * set every run takes one step per launch; a fused-pair rank grid refuses them.  *id (0, 1, ...) names the correlator; ids are
  * separate from the recorders' and injectors'.  Read-only option slice_correlator_launches: correlating launches since prepare
- * (one per step in which some correlator of this rank has a row due). */
+ * (one per step in which some correlator of this rank has a row due, and a second right after it when a correlator of
+ * yb_solution_add_slice_correlator_var has a row due in that step). */
 int yb_solution_add_slice_correlator(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
                                      int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id);
 /* The image of correlator `id` as the whole decimated box in the solution's type (0 where this rank owns no point) and the owned
  * mask, as yb_solution_get_slice_frames with one row. */
 int yb_solution_get_correlator_image(yb_solution* s, int64_t id, void* out, uint8_t* owned);
 int yb_solution_clear_slice_correlators(yb_solution* s);   /* remove every correlator and free its image; ids restart at 0 */
+
+/* A correlator as yb_solution_add_slice_correlator_typed whose b is var `src_var` of another prepared solution `src` on the same
+ * device, read at the paired step: when row r is due at step u,
+ *   image[pt] = I(image[pt] + var(u, pt) * src_var(src_t0 + (u - t0), pt)), rounded as yb_solution_add_slice_correlator_typed,
+ * at the same global points.  For a reverse-time shot with no snapshots: `src` rebuilds the source wavefield backwards in time
+ * beside the adjoint run `s`, and alternating one-step runs of the two enqueue with no host sync.  The two solutions may store
+ * their vars differently (pads, halos, slot counts, spare temporal-tile slots, another stencil).  Ids, image, image types,
+ * yb_solution_get_correlator_image, yb_solution_clear_slice_correlators and slice_correlator_launches are those of the other
+ * correlators.  All due correlators of this call share one launch per step, right after the launch of the other correlators,
+ * so a step in which both kinds are due takes two correlating launches.  Refused, naming the field, in this order: `src` is not another
+ * solution; `src_var` is missing or breaks the var rules of yb_solution_add_slice; the element bytes differ; the domain dims
+ * differ; (both with their rank geometry) the overall domain, rank grid or rank index differ; `src` is not prepared; the device
+ * differs (a consumer planned before its prepare is checked again then).  Ordering: every run of `s` waits for `src`'s last run
+ * and var-data writes, and every run or var-data write of `src` waits for the last run of `s`, so runs behave as if executed in
+ * the order the host enqueued them.  Before a run of `s` enqueues anything, every due step u of it must pair with a step inside
+ * the valid window of `src_var` as the host has enqueued `src` (yb_var_info first_valid_step .. last_valid_step); otherwise the
+ * run is refused, naming the correlator, u, the paired step and the window, and changes nothing.  If `src` is destroyed, the
+ * images stay readable and every run of `s` is refused until yb_solution_clear_slice_correlators. */
+int yb_solution_add_slice_correlator_var(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                         int64_t t0, int64_t every, int64_t nrows, yb_solution* src, const char* src_var, int64_t src_t0,
+                                         int image_type, int64_t* id);
 
 /* ---- frame and image types of the slice calls ------------------------------------------------------------------------
  * A recorder's or a host-fed injector's frames are held in a frame type F, and a correlator's image in an image type I.

@@ -66,7 +66,7 @@ ABI_SYMBOLS = [
     "yb_solution_add_slice_injector", "yb_solution_clear_slice_injectors", "yb_solution_add_slice_injector_from",
     "yb_solution_add_slice_correlator", "yb_solution_get_correlator_image", "yb_solution_clear_slice_correlators",
     "yb_solution_add_slice_typed", "yb_solution_add_slice_injector_typed", "yb_solution_add_slice_correlator_typed",
-    "yb_solution_get_slice_frame_type", "yb_solution_get_correlator_image_type",
+    "yb_solution_get_slice_frame_type", "yb_solution_get_correlator_image_type", "yb_solution_add_slice_correlator_var",
     "yb_halo_export_size", "yb_halo_export", "yb_halo_import", "yb_halo_finalize",
     "yb_exchange_halos", "yb_comm_env_rank", "yb_comm_env_world", "yb_comm_env_local_rank", "yb_comm_init", "yb_comm_rank", "yb_comm_world",
     "yb_comm_barrier", "yb_comm_allgather", "yb_comm_sum_i64", "yb_comm_max_f64", "yb_comm_finalize", "yb_halo_connect",
@@ -158,6 +158,8 @@ def lib() -> C.CDLL:
                                                            i32, i32, p, C.POINTER(i64)]
         L.yb_solution_add_slice_correlator_typed.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64,
                                                              p, i64, i32, i32, C.POINTER(i64)]
+        L.yb_solution_add_slice_correlator_var.argtypes = [p, C.c_char_p, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), i64, i64, i64,
+                                                           p, C.c_char_p, i64, i32, C.POINTER(i64)]
         L.yb_solution_get_slice_frame_type.argtypes = [p, i64, C.POINTER(i32)]
         L.yb_solution_get_correlator_image_type.argtypes = [p, i64, C.POINTER(i32)]
         L.yb_halo_export_size.argtypes = [p, C.POINTER(C.c_size_t)]
@@ -703,6 +705,25 @@ class Solution:
         _chk(lib().yb_solution_add_slice_correlator_typed(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
                                                           int(t0), int(every), int(nrows), None if src is None else src._h,
                                                           0 if src_id is None else int(src_id), int(reverse), itype, C.byref(rid)))
+        if not hasattr(self, "_correlators"):
+            self._correlators = {}
+        self._correlators[rid.value] = tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1)
+        return rid.value
+
+    def add_slice_correlator_var(self, var: str, first, last, t0: int, nrows: int, src: "Solution", src_var: str, src_t0: int = None,
+                                 stride=None, every: int = 1, image_dtype=None) -> int:
+        """add_slice_correlator whose b is var src_var of another prepared solution src on the same device, at the paired step:
+        when row r is due at step u, image += var(u) * src_var(src_t0 + (u - t0)) (src_t0 defaults to t0).  For a source wavefield
+        rebuilt backwards in time beside the adjoint run: alternating one-step runs of the two enqueue with no host sync and run
+        in the order they were called.  A run whose due steps pair with steps outside src_var's valid window, as src's calls have
+        left it, is refused before it changes anything.  Returns the correlator's id (shared with the other correlators)."""
+        itype = slice_type("slice correlator", "image_dtype", image_dtype)
+        f, l, st = self._box("slice correlator", first, last, stride)
+        rid = C.c_int64(-1)
+        _chk(lib().yb_solution_add_slice_correlator_var(self._h, var.encode(), _arr(f.tolist()), _arr(l.tolist()), _arr(st.tolist()),
+                                                        int(t0), int(every), int(nrows), None if src is None else src._h,
+                                                        None if src_var is None else src_var.encode(),
+                                                        int(t0 if src_t0 is None else src_t0), itype, C.byref(rid)))
         if not hasattr(self, "_correlators"):
             self._correlators = {}
         self._correlators[rid.value] = tuple(int(x) for x in (l - f) // np.maximum(st, 1) + 1)

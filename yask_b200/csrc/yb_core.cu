@@ -41,6 +41,7 @@ Solution::~Solution() {
         if (own_stream) cudaStreamDestroy(own_stream);
         if (comm_stream) cudaStreamDestroy(comm_stream);
     }
+    slices_source_gone(*this);   // consumers of this solution's vars (var links) refuse to run from now on
     points_free(points);     // device tables are released on `device`, selected above
     slices_free(slices);
     slices_free(injectors);
@@ -241,6 +242,8 @@ static int slice_copy(Solution& s, int var, void* buf, const int64_t* first, con
     int64_t done = 0;
     // chunk along the outermost box dim so the staging buffer stays bounded
     const size_t CHUNK = size_t(256) << 20;
+    if (to_var)
+        if (int rc = slices_var_write_waits(s)) return rc;
     for (int64_t t = sl.t0; t <= sl.t1; t++) {
         char* slot = v.slot_ptr(v.slot_of(t));
         char* hb = static_cast<char*>(buf) + size_t(t - sl.t0) * sl.elems_per_step * eb;
@@ -275,6 +278,8 @@ static int slice_copy(Solution& s, int var, void* buf, const int64_t* first, con
         done += sl.elems_per_step;
         if (to_var) v.update_valid_step(t);
     }
+    if (to_var)
+        if (int rc = slices_var_write_records(s)) return rc;
     if (to_var && s.halo) halo_mark_dirty(s, var);
     if (n_done) *n_done = done;
     return 0;
@@ -732,7 +737,9 @@ int yb_var_set_all_same(yb_solution* s_, int var, double value) {
     if (!s->prepared) return set_error(YB_ESTATE, "var storage is not allocated: call prepare_solution first");
     Var& v = s->vars[var];
     YB_CUDA(cudaSetDevice(s->device));
+    if (int rc = slices_var_write_waits(*s)) return rc;
     if (int rc = launch_fill_all(v.dev, v.slot_elems * v.nslots(), v.elem_bytes, value, s->stream())) return rc;
+    if (int rc = slices_var_write_records(*s)) return rc;
     if (s->halo) halo_mark_dirty(*s, var);
     return 0;
 }
@@ -745,10 +752,12 @@ int yb_var_set_slice_same(yb_solution* s_, int var, double value, const int64_t*
     Slice sl;
     if (int rc = resolve_slice(*s, v, first, last, false, sl)) return rc;
     YB_CUDA(cudaSetDevice(s->device));
+    if (int rc = slices_var_write_waits(*s)) return rc;
     for (int64_t t = sl.t0; t <= sl.t1; t++) {
         if (int rc = launch_box_fill(v.slot_ptr(v.slot_of(t)), sl.bc, v.elem_bytes, value, s->stream())) return rc;
         v.update_valid_step(t);
     }
+    if (int rc = slices_var_write_records(*s)) return rc;
     if (s->halo) halo_mark_dirty(*s, var);
     if (n_done) *n_done = sl.elems_per_step * (sl.t1 - sl.t0 + 1);
     return 0;
@@ -795,7 +804,9 @@ int yb_var_fill_hash_shifted(yb_solution* s_, int var, int64_t step, uint32_t se
             k++;
         }
     }
+    if (int rc = slices_var_write_waits(*s)) return rc;
     if (int rc = launch_hash_fill(v.slot_ptr(v.slot_of(step)), sl.bc, sl.g0, v.elem_bytes, seed, salt, lo, hi, s->stream())) return rc;
+    if (int rc = slices_var_write_records(*s)) return rc;
     v.update_valid_step(step);
     if (s->halo) halo_mark_dirty(*s, var);
     return 0;
@@ -850,7 +861,7 @@ int yb_solution_run(yb_solution* s_, int64_t first_step, int64_t last_step) {
     cudaStream_t st = s->stream();
     // point tables are normally uploaded when they are set (or at prepare); before anything of this run is enqueued otherwise
     if (int rc = points_begin_run(*s)) return rc;
-    if (int rc = slices_begin_run(*s)) return rc;
+    if (int rc = slices_begin_run(*s, first_step, last_step)) return rc;
     if (int rc = slices_run_waits(*s, st)) return rc;     // frames shared with other solutions (yb_slices.h)
     // Timing events: pairs of finished runs are folded into the stats and recycled here, so that calling
     // run_solution(t) once per step (the reference's usual pattern) keeps a bounded number of events alive.

@@ -3,8 +3,8 @@
 // get_elements_in_slice, which pays a synchronous device-to-host copy per frame and loses the temporal tile's pairs.  Slice
 // injectors write boxes back the same way (plane-wave and areal sources, boundary replay, time-varying Dirichlet data), instead of
 // the loop run_solution(t, t) / get_elements_in_slice / set_elements_in_slice.  Slice correlators accumulate the imaging condition
-// image += var(u) * frame into an image on the device, the frames being var(u) itself or a recorder's, instead of the loop
-// run_solution(t, t) / get_elements_in_slice / host arithmetic.
+// image += var(u) * b into an image on the device, b being var(u) itself, a recorder's frame or a var of another solution at a
+// paired step, instead of the loop run_solution(t, t) / get_elements_in_slice / host arithmetic.
 #include <stdio.h>
 #include <string.h>
 
@@ -37,6 +37,11 @@ struct SliceDesc {
     int mode;
     long long loc0[4], lstep[4];
     int ftype, itype;               // YB_TYPE_* of the frames and (correlators) of the image; never YB_TYPE_ELEM
+    // correlators with a var link (b_var): b is element b_off + c0 * b_vs[0] + c1 * b_vs[1] + c2 * b_vs[2] + i * b_vs[3] of the
+    // source var's slot imod(u + b_shift, b_alloc) + b_bias (b_slot_bytes each) at box index (c0, c1, c2, i)
+    const char* b_base;
+    long long b_slot_bytes, b_shift, b_off, b_vs[4];
+    int b_var, b_alloc, b_bias;
 };
 
 // A 16-bit frame element, held as its bit pattern.
@@ -182,14 +187,14 @@ __device__ __forceinline__ double mul_add_rn(double img, float v, float b) { ret
 // threads walk rows of the unit-stride dim, 2^lanes_log2 threads per row: a row's storage offset is computed once, with the two
 // 64-bit divisions that split the row index, and the lanes step along it, so a full-volume correlator reads var, frame and image
 // contiguously and stays bound by memory, not by per-point index arithmetic.  Offsets are 64-bit: a slot may hold more than 2^31
-// elements.
+// elements.  Var links (b_var) are left to slice_correlators_var_kernel.
 template <typename T>
 __global__ void __launch_bounds__(256) slice_correlators_kernel(const SliceDesc* __restrict__ table, int n, long long t) {
     for (int r = blockIdx.y; r < n; r += gridDim.y) {
         const SliceDesc& d = table[r];
         const long long u = t + d.step_off;
         long long row;
-        if (!row_due(u, d.t0, d.every, d.nrows, row)) continue;
+        if (d.b_var || !row_due(u, d.t0, d.every, d.nrows, row)) continue;
         const BoxDev b = d.box;
         long long slot = u % d.alloc;
         slot = (slot < 0 ? slot + d.alloc : slot) + d.bias;
@@ -226,8 +231,46 @@ __global__ void __launch_bounds__(256) slice_correlators_kernel(const SliceDesc*
     }
 }
 
-// The x grid is a grid-stride cap: 8 CTAs per SM is two waves at the 4 CTAs of 256 threads per SM that the kernel's 56
-// registers allow.  y: the hardware limit of gridDim.y; more recorders are walked by the y loop.
+__device__ __forceinline__ long long slot_at(long long u, int alloc, int bias) {
+    const long long c = u % alloc;
+    return (c < 0 ? c + alloc : c) + bias;
+}
+
+// The var links of the table (b_var): slice_correlators_kernel's row walk, with b read in T from the source var's step slot of
+// the paired step through the descriptor's strides, so the source may store its var with other pads, halos and slots.  A kernel
+// of its own: the second set of 64-bit row strides does not fit in slice_correlators_kernel's 64 registers.
+template <typename T>
+__global__ void __launch_bounds__(256) slice_correlators_var_kernel(const SliceDesc* __restrict__ table, int n, long long t) {
+    for (int r = blockIdx.y; r < n; r += gridDim.y) {
+        const SliceDesc& d = table[r];
+        const long long u = t + d.step_off;
+        long long row;
+        if (!d.b_var || !row_due(u, d.t0, d.every, d.nrows, row)) continue;
+        const BoxDev b = d.box;
+        const T* __restrict__ var = reinterpret_cast<const T*>(d.var_base + slot_at(u, d.alloc, d.bias) * d.slot_bytes) + b.off;
+        const T* __restrict__ src = reinterpret_cast<const T*>(d.b_base + slot_at(u + d.b_shift, d.b_alloc, d.b_bias) * d.b_slot_bytes) + d.b_off;
+        const int lg = d.lanes_log2, lanes = 1 << lg;
+        const long long len = b.n[3], vs = b.vs[3], bs = d.b_vs[3], rows = b.n[0] * b.n[1] * b.n[2], per = 256 >> lg;
+        const int lane = threadIdx.x & (lanes - 1);
+        auto walk = [&](auto itag) {
+            using I = decltype(itag);
+            I* __restrict__ img = reinterpret_cast<I*>(d.image);
+            for (long long q = blockIdx.x * per + (threadIdx.x >> lg); q < rows; q += gridDim.x * per) {
+                const long long q1 = q / b.n[2], c2 = q - q1 * b.n[2];
+                const long long c0 = q1 / b.n[1], c1 = q1 - c0 * b.n[1];
+                const T* __restrict__ vrow = var + c0 * b.vs[0] + c1 * b.vs[1] + c2 * b.vs[2];
+                const T* __restrict__ brow = src + c0 * d.b_vs[0] + c1 * d.b_vs[1] + c2 * d.b_vs[2];
+                const long long o = q * len;
+                for (long long i = lane; i < len; i += lanes) img[o + i] = mul_add_rn(img[o + i], vrow[i * vs], brow[i * bs]);
+            }
+        };
+        if (sizeof(T) == 4 && d.itype == YB_TYPE_F64) walk(double{});
+        else walk(T{});
+    }
+}
+
+// The x grid is a grid-stride cap: 8 CTAs per SM is two waves at the 4 CTAs of 256 threads per SM that the kernels' 64 registers
+// allow (slice_correlators_var_kernel<float>, at 76, fits 3).  y: the hardware limit of gridDim.y; more recorders are walked by the y loop.
 constexpr int CTAS_PER_SM = 8, MAX_GRID_Y = 65535;
 
 // A device buffer freed with cudaFree on its device by its last holder: a recorder's frames outlive the recorder, and its solution,
@@ -301,6 +344,49 @@ int check_link(const Solution& s, const SlicesState& p, const SliceRec& r) {
     return 0;
 }
 
+// A var link's source against the consumer s, attach checks 3 to 7 of yb_solution_add_slice_correlator_var in their order: element
+// bytes, domain dims, then (both with their rank geometry) overall domain, rank grid and rank index, then that src is prepared,
+// and on a consumer with a device, the device.  Each refusal names the field that differs.
+int check_var_src(const Solution& s, const char* what, const Solution& src) {
+    if (src.spec.elem_bytes != s.spec.elem_bytes)
+        return set_error(YB_EINVAL, "%s: element bytes %d differ from the source solution's %d", what, s.spec.elem_bytes, src.spec.elem_bytes);
+    if (src.ndd != s.ndd)
+        return set_error(YB_EINVAL, "%s: %d domain dims differ from the source solution's %d", what, s.ndd, src.ndd);
+    for (int k = 0; k < s.ndd; k++)
+        if (src.spec.domain_dims[k] != s.spec.domain_dims[k])
+            return set_error(YB_EINVAL, "%s: domain dim %d '%s' differs from the source solution's '%s'", what, k, s.spec.domain_dims[k].c_str(),
+                             src.spec.domain_dims[k].c_str());
+    if (!geometry_known(s)) return set_error(YB_ESTATE, "%s: this solution has no rank geometry yet (plan_geometry / prepare_solution)", what);
+    if (!geometry_known(src))
+        return set_error(YB_ESTATE, "%s: the source solution has no rank geometry yet (plan_geometry / prepare_solution)", what);
+    for (int k = 0; k < s.ndd; k++)
+        if (s.overall_size[k] != src.overall_size[k])
+            return set_error(YB_EINVAL, "%s: overall domain size %lld in dim '%s' differs from the source solution's %lld", what,
+                             (long long)s.overall_size[k], s.spec.domain_dims[k].c_str(), (long long)src.overall_size[k]);
+    for (int k = 0; k < s.ndd; k++)
+        if (s.num_ranks[k] != src.num_ranks[k])
+            return set_error(YB_EINVAL, "%s: num_ranks %lld in dim '%s' differs from the source solution's %lld (rank grid)", what,
+                             (long long)s.num_ranks[k], s.spec.domain_dims[k].c_str(), (long long)src.num_ranks[k]);
+    for (int k = 0; k < s.ndd; k++)
+        if (s.rank_index[k] != src.rank_index[k])
+            return set_error(YB_EINVAL, "%s: rank index %lld in dim '%s' differs from the source solution's %lld", what,
+                             (long long)s.rank_index[k], s.spec.domain_dims[k].c_str(), (long long)src.rank_index[k]);
+    if (!src.prepared)
+        return set_error(YB_ESTATE, "%s: the source solution '%s' is not prepared, so its vars have no storage yet", what, src.spec.name.c_str());
+    if (s.device >= 0 && s.device != src.device)
+        return set_error(YB_EINVAL, "%s: device %d differs from the source solution's device %d", what, s.device, src.device);
+    return 0;
+}
+
+// A var link at plan and prepare: the source still exists and still passes check_var_src.
+int check_var_link(const Solution& s, const SlicesState& p, const SliceRec& r) {
+    const FrameLink& l = *r.link;
+    if (!l.src)
+        return set_error(YB_ESTATE, "%s: the source solution '%s' of var '%s' was destroyed", p.what, l.src_name.c_str(),
+                         s.vars[r.var].spec.name.c_str());
+    return check_var_src(s, p.what, *l.src);
+}
+
 // this rank's part of one recorder, injector or correlator; refuses a box outside the overall domain, on a rank grid an injector
 // into a var the last stage does not write (it must land before that stage's exchange, as a source does), and a consumer whose
 // part differs from its recorder's (check_link)
@@ -329,7 +415,7 @@ int plan_one(const Solution& s, const SlicesState& p, SliceRec& r) {
         const Dim* d = v.domain_dim(k);
         r.own_off += (r.first[k] + k0 * st - lo + d->pad_l) * d->stride;
     }
-    return r.link ? check_link(s, p, r) : 0;
+    return r.link ? (r.link->var_link ? check_var_link(s, p, r) : check_link(s, p, r)) : 0;
 }
 
 // rank-local coordinate of the first owned point in domain dim k (the last one is that + (own_n[k] - 1) * stride[k])
@@ -372,6 +458,11 @@ int lanes_log2(int64_t len) {
     return lg;
 }
 
+// the source var of a var link whose source still exists, else null
+const Var* link_var(const SliceRec& r) {
+    return r.link && r.link->var_link && r.link->src ? &r.link->src->vars[size_t(r.link->src_var)] : nullptr;
+}
+
 SliceDesc describe(const Solution& s, const SliceRec& r) {
     const Var& v = s.vars[r.var];
     SliceDesc d{};
@@ -398,6 +489,22 @@ SliceDesc describe(const Solution& s, const SliceRec& r) {
     d.lanes_log2 = lanes_log2(d.box.n[3]);
     d.ftype = r.ftype;
     d.itype = r.itype;
+    // a var link: b from the source var, with the consumer's rank geometry (check_var_src) but its own pads, strides and slots;
+    // none once the source is gone (slices_begin_run then refuses every run)
+    if (!r.link || !r.link->var_link) return d;
+    d.b_var = 1;
+    const Var* bv = link_var(r);
+    if (!bv) return d;
+    d.b_base = static_cast<const char*>(bv->dev);
+    d.b_slot_bytes = (long long)bv->slot_elems * bv->elem_bytes;
+    d.b_alloc = bv->step_alloc();
+    d.b_bias = bv->slot_bias;
+    d.b_shift = r.link->src_shift;
+    for (int k = 0; k < s.ndd; k++) {
+        const Dim* bd = bv->domain_dim(k);
+        d.b_off += (r.first[k] + r.own_k0[k] * r.stride[k] - s.rank_offset[k] + bd->pad_l) * bd->stride;
+        d.b_vs[4 - s.ndd + k] = bd->stride * r.stride[k];
+    }
     return d;
 }
 
@@ -459,6 +566,10 @@ int upload_table(Solution& s, SlicesState& p) {
         t.push_back(describe(s, r));
         r.uploaded_bias = s.vars[r.var].slot_bias;
         r.uploaded_base = s.vars[r.var].dev;
+        if (const Var* bv = link_var(r)) {
+            r.uploaded_src_bias = bv->slot_bias;
+            r.uploaded_src_base = bv->dev;
+        }
     }
     if (t.empty()) return 0;
     YB_CUDA(cudaDeviceGetAttribute(&p.num_sms, cudaDevAttrMultiProcessorCount, s.device));
@@ -516,11 +627,44 @@ int prepare_state(Solution& s, SlicesState* p) {
     return upload_table(s, *p);
 }
 
-int begin_run_state(Solution& s, SlicesState* p) {
+// A var link's pairings in a run of steps first .. last: the due steps u of the run form an arithmetic sequence, and so do their
+// source steps u + src_shift, so the first and last due steps bound them against the source var's valid window (as the source's
+// host calls have enqueued it: the source cannot advance while this run is in flight).  Checked in run order.
+int check_pairs(const Solution& s, const SlicesState& p, size_t id, const SliceRec& r, int64_t first, int64_t last) {
+    const FrameLink& l = *r.link;
+    if (!l.src)
+        return set_error(YB_ESTATE, "%s %zu: its source solution '%s' was destroyed; no run is possible until clear_slice_correlators()",
+                         p.what, id, l.src_name.c_str());
+    const Var& bv = l.src->vars[size_t(l.src_var)];
+    const int64_t lo = std::min(first, last) + r.step_off, hi = std::max(first, last) + r.step_off;
+    const int64_t k0 = std::max<int64_t>(0, lo - r.t0 <= 0 ? 0 : (lo - r.t0 + r.every - 1) / r.every);
+    const int64_t k1 = hi < r.t0 ? -1 : std::min<int64_t>(r.nrows - 1, (hi - r.t0) / r.every);
+    if (k0 > k1) return 0;
+    const int64_t ua = r.t0 + k0 * r.every, ub = r.t0 + k1 * r.every;
+    const int64_t order[2] = {last >= first ? ua : ub, last >= first ? ub : ua};
+    for (int64_t u : order) {
+        const int64_t w = u + l.src_shift;
+        if (w < bv.first_valid_step || w > bv.last_valid_step())
+            return set_error(YB_ERANGE, "%s %zu: step %lld pairs with step %lld of var '%s' of the source solution '%s', outside its valid "
+                             "steps [%lld, %lld]", p.what, id, (long long)u, (long long)w, bv.spec.name.c_str(), l.src_name.c_str(),
+                             (long long)bv.first_valid_step, (long long)bv.last_valid_step());
+    }
+    return 0;
+}
+
+int begin_run_state(Solution& s, SlicesState* p, int64_t first, int64_t last) {
     if (!active(p)) return 0;
     if (int rc = check_mode(s, *p)) return rc;
     bool moved = false;
-    for (auto& r : p->recs) moved = moved || r.uploaded_bias != s.vars[r.var].slot_bias || r.uploaded_base != s.vars[r.var].dev;
+    for (size_t i = 0; i < p->recs.size(); i++) {
+        const SliceRec& r = p->recs[i];
+        if (r.link && r.link->var_link)
+            if (int rc = check_pairs(s, *p, i, r, first, last)) return rc;
+    }
+    for (auto& r : p->recs) {
+        moved = moved || r.uploaded_bias != s.vars[r.var].slot_bias || r.uploaded_base != s.vars[r.var].dev;
+        if (const Var* bv = link_var(r)) moved = moved || r.uploaded_src_bias != bv->slot_bias || r.uploaded_src_base != bv->dev;
+    }
     if (!moved) return 0;
     YB_CUDA(cudaStreamSynchronize(s.stream()));
     return upload_table(s, *p);
@@ -565,6 +709,8 @@ void slices_preload() {
     preload_kernel((const void*)slice_injectors_kernel<double>);
     preload_kernel((const void*)slice_correlators_kernel<float>);
     preload_kernel((const void*)slice_correlators_kernel<double>);
+    preload_kernel((const void*)slice_correlators_var_kernel<float>);
+    preload_kernel((const void*)slice_correlators_var_kernel<double>);
 }
 
 bool slices_active(const Solution& s) { return active(s.slices); }
@@ -585,9 +731,32 @@ int slices_prepare(Solution& s) {
     return 0;
 }
 
-int slices_begin_run(Solution& s) {
+int slices_begin_run(Solution& s, int64_t first_step, int64_t last_step) {
     for (SlicesState* p : {s.slices, s.injectors, s.correlators})
-        if (int rc = begin_run_state(s, p)) return rc;
+        if (int rc = begin_run_state(s, p, first_step, last_step)) return rc;
+    return 0;
+}
+
+void slices_source_gone(Solution& s) {
+    if (s.slices)
+        for (const auto& w : s.slices->readers)
+            if (auto l = w.lock())
+                if (l->var_link) l->src = nullptr;
+}
+
+int slices_var_write_waits(Solution& s) {
+    if (s.slices)
+        for (const auto& w : s.slices->readers)
+            if (auto l = w.lock())
+                if (l->var_link) YB_CUDA(cudaStreamWaitEvent(s.stream(), l->read, 0));
+    return 0;
+}
+
+int slices_var_write_records(Solution& s) {
+    if (s.slices)
+        for (const auto& w : s.slices->readers)
+            if (auto l = w.lock())
+                if (l->var_link) YB_CUDA(cudaEventRecord(l->written, s.stream()));
     return 0;
 }
 
@@ -634,22 +803,28 @@ int slices_launch(Solution& s, int64_t t, cudaStream_t st) {
 int slice_correlators_launch(Solution& s, int64_t t, cudaStream_t st) {
     if (!slice_correlators_active(s)) return 0;
     SlicesState& p = *s.correlators;
-    int64_t most = 0;
+    int64_t most[2] = {0, 0};         // frame and autocorrelation correlators; var links
     for (auto& r : p.recs) {
         long long row;
         if (!r.own_elems || !row_due(t + r.step_off, r.t0, r.every, r.nrows, row)) continue;
         // the CTAs this correlator's rows fill, 256 >> lanes_log2 rows per CTA
         const int64_t len = r.own_n[s.ndd - 1], per = 256 >> lanes_log2(len);
-        most = std::max(most, (r.own_elems / len + per - 1) / per);
+        int64_t& m = most[r.link && r.link->var_link];
+        m = std::max(m, (r.own_elems / len + per - 1) / per);
     }
-    if (!most) return 0;
-    const dim3 grid(unsigned(std::min<int64_t>(most, int64_t(p.num_sms) * CTAS_PER_SM)), unsigned(std::min<size_t>(p.recs.size(), MAX_GRID_Y)));
     const SliceDesc* table = static_cast<const SliceDesc*>(p.d_table);
-    if (s.spec.elem_bytes == 4) slice_correlators_kernel<float><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
-    else slice_correlators_kernel<double><<<grid, 256, 0, st>>>(table, int(p.recs.size()), t);
-    YB_CUDA(cudaGetLastError());
-    p.launches++;
-    return 1;
+    const int n = int(p.recs.size());
+    int launched = 0;
+    for (int k = 0; k < 2; k++) {
+        if (!most[k]) continue;
+        const dim3 grid(unsigned(std::min<int64_t>(most[k], int64_t(p.num_sms) * CTAS_PER_SM)), unsigned(std::min(n, MAX_GRID_Y)));
+        if (s.spec.elem_bytes == 4) (k ? slice_correlators_var_kernel<float> : slice_correlators_kernel<float>)<<<grid, 256, 0, st>>>(table, n, t);
+        else (k ? slice_correlators_var_kernel<double> : slice_correlators_kernel<double>)<<<grid, 256, 0, st>>>(table, n, t);
+        YB_CUDA(cudaGetLastError());
+        p.launches++;
+        launched++;
+    }
+    return launched;
 }
 
 int slice_injectors_launch(Solution& s, int64_t t, int sel, const Box& interior, cudaStream_t st) {
@@ -831,9 +1006,15 @@ static int clear_state(Solution* s, SlicesState*& p, SliceKind kind) {
         YB_CUDA(cudaStreamSynchronize(s->stream()));
     }
     const int64_t launches = p->launches;
+    // the var links of consumers of this solution's vars stay ordered against its runs
+    std::vector<std::weak_ptr<FrameLink>> keep;
+    for (const auto& w : p->readers)
+        if (auto l = w.lock())
+            if (l->var_link) keep.push_back(w);
     slices_free(p);
     p = new_state(kind);
     p->launches = launches;
+    p->readers = std::move(keep);
     return 0;
 }
 
@@ -937,6 +1118,47 @@ int yb_solution_add_slice_correlator_typed(yb_solution* s_, const char* var, con
 int yb_solution_add_slice_correlator(yb_solution* s, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
                                      int64_t t0, int64_t every, int64_t nrows, yb_solution* src, int64_t src_id, int reverse, int64_t* id) {
     return yb_solution_add_slice_correlator_typed(s, var, first, last, stride, t0, every, nrows, src, src_id, reverse, YB_TYPE_ELEM, id);
+}
+
+int yb_solution_add_slice_correlator_var(yb_solution* s_, const char* var, const int64_t* first, const int64_t* last, const int64_t* stride,
+                                         int64_t t0, int64_t every, int64_t nrows, yb_solution* src_, const char* src_var, int64_t src_t0,
+                                         int image_type, int64_t* id) {
+    Solution* s = SOL(s_);
+    if (!s) return set_error(YB_EINVAL, "null solution");
+    const char* what = "slice correlator";
+    SliceRec r;
+    int64_t bytes = 0;
+    if (int rc = new_rec(s, what, var, first, last, stride, t0, every, nrows, YB_TYPE_ELEM, r, bytes)) return rc;
+    if (int rc = resolve_type(*s, what, image_type, true, r.itype)) return rc;
+    Solution* src = SOL(src_);
+    if (!src) return set_error(YB_EINVAL, "%s: src: null source solution", what);
+    if (src == s) return set_error(YB_EINVAL, "%s: src: the source solution must be another solution, not this one", what);
+    int src_vi = -1, src_off = 0;
+    if (int rc = point_var(*src, "slice correlator: src_var", src_var, src_vi, src_off)) return rc;
+    if (!s->correlators) s->correlators = new_state(SLICE_CORRELATE);
+    if (int rc = check_mode(*s, *s->correlators)) return rc;
+    if (int rc = check_var_src(*s, what, *src)) return rc;
+    auto link = std::make_shared<FrameLink>();
+    link->device = src->device;
+    link->elem_bytes = src->spec.elem_bytes;
+    link->ndd = src->ndd;
+    link->var_link = true;
+    link->src = src;
+    link->src_var = src_vi;
+    link->src_shift = src_t0 - t0;
+    link->src_name = src->spec.name;
+    r.link = link;
+    if (int rc = plan_one(*s, *s->correlators, r)) return rc;
+    // the events that order the two streams, created here (run_solution() allocates nothing)
+    YB_CUDA(cudaSetDevice(src->device));
+    YB_CUDA(cudaEventCreateWithFlags(&link->written, cudaEventDisableTiming));
+    YB_CUDA(cudaEventCreateWithFlags(&link->read, cudaEventDisableTiming));
+    YB_CUDA(cudaEventRecord(link->written, src->stream()));     // the source's work enqueued so far
+    if (!src->slices) src->slices = new_state(SLICE_RECORD);    // holds the readers even with no recorder
+    auto& readers = src->slices->readers;
+    readers.erase(std::remove_if(readers.begin(), readers.end(), [](const std::weak_ptr<FrameLink>& w) { return w.expired(); }), readers.end());
+    readers.push_back(link);
+    return install(s, s->correlators, SLICE_CORRELATE, std::move(r), id);
 }
 
 int yb_solution_get_slice_frame_type(yb_solution* s_, int64_t id, int* type) {

@@ -14,7 +14,9 @@
 //
 // A correlator has a recorder's box and window and accumulates var(u) * b into an image of one frame, on the device: b is var(u)
 // itself (autocorrelation: the source illumination) or row r, or nrows - 1 - r (reverse), of a recorder's frames.  Correlators
-// run after the step's recorders.  Injectors may read a recorder's frames the same way instead of the caller's.
+// run after the step's recorders.  Injectors may read a recorder's frames the same way instead of the caller's.  A correlator may
+// also read b from a var of another prepared solution on the same device, at the paired step src_t0 + (u - t0) (a var link): the
+// source wavefield rebuilt backwards in time beside the adjoint run, so the shot stores no snapshots.
 #pragma once
 #include <memory>
 
@@ -24,7 +26,9 @@ namespace yb {
 
 // A recorder's frames held by a consumer (a correlator, or an injector fed from a recorder): the geometry the attach call checked,
 // checked again at the consumer's prepare, and the events that order the two solutions' streams -- none when the source is the
-// consumer itself.  Held by the consumer; the source keeps a weak reference (SlicesState::readers).
+// consumer itself.  Held by the consumer; the source keeps a weak reference (SlicesState::readers).  A var link (src non-null:
+// a correlator reading a var of another solution) names the source and its var instead of a recorder; the source's destructor
+// clears src (slices_source_gone), after which the consumer refuses to run until its correlators are cleared.
 struct FrameLink {
     int device = -1, elem_bytes = 0, ndd = 0;
     int ftype = 0;                              // the recorder's frame type (YB_TYPE_*), which the consumer reads
@@ -34,6 +38,12 @@ struct FrameLink {
     int64_t own_k0[3] = {0, 0, 0}, own_n[3] = {0, 0, 0};
     cudaEvent_t written = nullptr;              // recorded by the source after each of its runs
     cudaEvent_t read = nullptr;                 // recorded by the consumer after each of its runs
+    // var links only
+    bool var_link = false;
+    Solution* src = nullptr;                    // null once the source is destroyed
+    int src_var = -1;
+    int64_t src_shift = 0;                      // source step = consumer step u + src_shift (src_t0 - t0)
+    std::string src_name;                       // the source solution's name, for messages after it is gone
     ~FrameLink();
 };
 
@@ -54,6 +64,8 @@ struct SliceRec {
     // the var's storage and slot_bias as the device table holds them (fuse_vars and the offline tuner's pairs move them)
     const void* uploaded_base = nullptr;
     int uploaded_bias = -1;
+    const void* uploaded_src_base = nullptr;    // the same of a var link's source var
+    int uploaded_src_bias = -1;
     // injectors only
     int mode = 0;                               // YB_INJECT_ADD / YB_INJECT_SET
     std::vector<char> host_frames;              // the caller's frames (nrows x the whole decimated box) until uploaded
@@ -76,7 +88,9 @@ struct SlicesState {
     int num_sms = 0;                            // of the solution's device, read with the table
     int64_t launches = 0;                       // launches since prepare (read-only options slice_launches, slice_injector_launches)
     std::vector<int> group_first;               // injectors: launch group g is recs[group_first[g] .. group_first[g + 1])
-    std::vector<std::weak_ptr<FrameLink>> readers;   // recorders: consumers in other solutions, which this one's runs order
+    // recorders: consumers in other solutions of this one's frames or vars (var links), which this one's runs order; the var
+    // links outlive clear_slices
+    std::vector<std::weak_ptr<FrameLink>> readers;
 };
 
 void slices_free(SlicesState* p);
@@ -89,9 +103,17 @@ int slices_plan(Solution& s);
 // plan, then allocate the frames of every recorder and injector, the images of the correlators, and upload the descriptor tables
 // (prepare_solution)
 int slices_prepare(Solution& s);
-// before a run enqueues anything: refresh the descriptor tables if a var's storage (fuse_vars) or live slots (a temporal tile
-// of the offline tuner) moved since they were uploaded; never allocates a frame buffer
-int slices_begin_run(Solution& s);
+// before a run of steps first_step .. last_step enqueues anything: refuse it if a correlator's var link has lost its source or
+// pairs a due step with a source step outside the source var's valid window; then refresh the descriptor tables if a var's
+// storage (fuse_vars) or live slots (a temporal tile of the offline tuner) moved since they were uploaded, a var link's source
+// var included; never allocates a frame buffer
+int slices_begin_run(Solution& s, int64_t first_step, int64_t last_step);
+// The source solution s is being destroyed: its var links' consumers lose it (FrameLink::src)
+void slices_source_gone(Solution& s);
+// Writes of the var-data calls into s's vars (fills, set_elements): before them s's stream waits for the last runs of the
+// consumers that read its vars (var links), and after them records the event those consumers' next runs wait on.
+int slices_var_write_waits(Solution& s);
+int slices_var_write_records(Solution& s);
 // Frames shared between two solutions: at the start of a run, before anything else is enqueued, the stream waits for the
 // sources' last runs to have written the frames this solution reads, and for its consumers' last runs to have read the frames
 // this solution writes; at its end the run records its own events for them.  Never allocates.

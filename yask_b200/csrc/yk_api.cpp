@@ -1172,6 +1172,23 @@ idx_t yk_add_slice_correlator_typed(yk_solution_ptr soln, const std::string& var
     return idx_t(id);
 }
 
+idx_t yk_add_slice_correlator_var(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                  idx_t nrows, yk_solution_ptr src, const std::string& src_var, idx_t src_t0, const idx_t_vec& stride,
+                                  idx_t every, const std::string& image_dtype) {
+    B200Solution& s = b200_slices(soln);
+    std::vector<int64_t> f, l, st;
+    slice_box(s, "slice correlator", first, last, stride, f, l, st);
+    const int type = slice_type("slice correlator", "image_dtype", image_dtype);
+    int64_t id = -1;
+    chk(yb_solution_add_slice_correlator_var(s.h->s, var.c_str(), f.data(), l.data(), st.empty() ? nullptr : st.data(), t0, every, nrows,
+                                             src ? b200_slices(src).h->s : nullptr, src_var.c_str(), src_t0, type, &id));
+    idx_t_vec shape;
+    for (size_t k = 0; k < f.size(); k++) shape.push_back((l[k] - f[k]) / (st.empty() ? 1 : st[k]) + 1);
+    s.correlator_shape.resize(size_t(id) + 1);
+    s.correlator_shape[size_t(id)] = shape;
+    return idx_t(id);
+}
+
 void yk_get_correlator_image(yk_solution_ptr soln, idx_t id, std::vector<double>& image, idx_t_vec& shape, std::vector<bool>& owned) {
     B200Solution& s = b200_slices(soln);
     if (id < 0 || size_t(id) >= s.correlator_shape.size()) fail("get_correlator_image: no slice correlator " + std::to_string(id));

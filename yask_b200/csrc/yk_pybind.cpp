@@ -329,6 +329,9 @@ PYBIND11_MODULE(yask_kernel, m) {
     m.def("yk_add_slice_correlator", &yk_add_slice_correlator, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
           py::arg("t0"), py::arg("nrows"), py::arg("src") = yk_solution_ptr(), py::arg("src_id") = 0, py::arg("reverse") = false,
           py::arg("stride") = idx_t_vec{}, py::arg("every") = 1);
+    m.def("yk_add_slice_correlator_var", &yk_add_slice_correlator_var, py::arg("soln"), py::arg("var"), py::arg("first"), py::arg("last"),
+          py::arg("t0"), py::arg("nrows"), py::arg("src"), py::arg("src_var"), py::arg("src_t0"), py::arg("stride") = idx_t_vec{},
+          py::arg("every") = 1, py::arg("image_dtype") = "");
     m.def("yk_get_correlator_image", [](yk_solution_ptr s, idx_t id) {
         std::vector<double> image;
         idx_t_vec shape;

@@ -62,12 +62,20 @@ idx_t yk_add_slice_injector_from(yk_solution_ptr soln, const std::string& var, c
 idx_t yk_add_slice_correlator(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
                               idx_t nrows, yk_solution_ptr src = nullptr, idx_t src_id = 0, bool reverse = false,
                               const idx_t_vec& stride = {}, idx_t every = 1);
+// A correlator whose b is var src_var of another prepared solution src on the same device at the paired step: image += var(u) *
+// src_var(src_t0 + (u - t0)), for a source wavefield rebuilt backwards in time beside the adjoint run instead of stored as
+// snapshots.  Semantics, checks and ordering: yb_solution_add_slice_correlator_var in include/yask_b200.h.  Shares the ids,
+// getters and launch counter of the other correlators.
+idx_t yk_add_slice_correlator_var(yk_solution_ptr soln, const std::string& var, const idx_t_vec& first, const idx_t_vec& last, idx_t t0,
+                                  idx_t nrows, yk_solution_ptr src, const std::string& src_var, idx_t src_t0, const idx_t_vec& stride = {},
+                                  idx_t every = 1, const std::string& image_dtype = "");
 // image: the decimated box, row-major, the last domain dim fastest, widened to double (points this rank does not own are 0);
 // shape: the box extents; owned: per box point, this rank holds it.
 void yk_get_correlator_image(yk_solution_ptr soln, idx_t id, std::vector<double>& image, idx_t_vec& shape, std::vector<bool>& owned);
 // Remove every correlator and free its image.
 void yk_clear_slice_correlators(yk_solution_ptr soln);
-// Correlating launches since prepare_solution().
+// Correlating launches since prepare_solution(): one per step with a row due, and a second right after it when a correlator with a
+// source var (yk_add_slice_correlator_var) has a row due too.
 idx_t yk_get_slice_correlator_launches(yk_solution_ptr soln);
 
 // Frame and image types (the typed calls): "float16", "bfloat16", "float32" or "float64"; "" is the element type.  Allowed
