@@ -135,9 +135,9 @@ def x_halo(ir):
     return max(max(v["halo"].get(d0, [0, 0])) for v in ir["vars"])
 
 
-# ---- the direct kernels' y chunking (yb_gen.cu:383-401), restated ----------------------------------------------------
+# ---- the direct kernels' y chunking (yb_gen.cu:388-406), restated ----------------------------------------------------
 def _pad_alloc(ir, k, n, align_elems):
-    """Allocated extent of domain dim k: every var is padded to the largest halo any var has there (yb_gen.cu:441-443);
+    """Allocated extent of domain dim k: every var is padded to the largest halo any var has there (yb_gen.cu:446-448);
     the unit-stride dim's left pad and pitch are rounded up to 128 bytes (yb_core.cu:102-110)."""
     d = ir["domain_dims"][k]
     u = max(max(v["halo"].get(d, [0, 0])) for v in ir["vars"])
@@ -166,7 +166,7 @@ def _launch_box(part, n):
 
 def direct_ychunks(name, n, l2_mb):
     """Per non-scratch part of a 3-D solution: (nyb, ychunk) of its direct kernel at option gen_l2_mb = l2_mb, as
-    GenEngine::launch (yb_gen.cu:383-401) computes them: the y chunk keeps (2 x halo + 1) x planes of every distinct
+    GenEngine::launch (yb_gen.cu:388-406) computes them: the y chunk keeps (2 x halo + 1) x planes of every distinct
     full-rank var the part touches within the L2 budget, at least 4 y blocks, and the chunks are equalised."""
     ir = ir_of(name)
     eb = ir["elem_bytes"]

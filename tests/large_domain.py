@@ -16,6 +16,15 @@ from yask_b200.synth import hash_field, var_salt
 
 TWO31 = 1 << 31
 
+# (below, at) sizes of the generated kernels' switch to 64-bit positions (GenEngine::prepare), for the switch-point cases of
+# tests/test_generated_wide_gpu.py: the largest var slot lies under 2^31 elements by less than one x plane, then at or above
+# 2^31 by less than one x plane.  At the "at" size 2^31 falls inside the last x pad plane, so only the high corner's x
+# neighbours read past it.  tests/test_generated_wide_cpu.py checks both from plan_geometry().
+SWITCH_SIZES = {
+    "3axis": ((1416, 1200, 1200), (1417, 1200, 1200)),
+    "test_2d": ((45644, 47000), (45645, 47000)),
+}
+
 
 class Window:
     """Oracle window [lo, lo + size) of a global domain of size n, trimmed by the cone rule to the kept box [kept_lo, kept_hi)."""

@@ -87,7 +87,7 @@ def test_grid_rows_cover_what_the_older_rank_grid_test_leaves():
 def test_l2_chunking_size_really_chunks(name):
     """At gen_l2_mb = 1 the direct kernels of these rows run in y chunks, the last one shorter: the y-chunked CTA order of
     gen_block_coords (yb_gen.cuh:140-152) with its `min(ychunk, nyb - y0)` branch.  G.direct_ychunks restates
-    yb_gen.cu:383-401; if the engine's formula changes, this names the row that no longer chunks."""
+    yb_gen.cu:388-406; if the engine's formula changes, this names the row that no longer chunks."""
     r = G.BY_NAME[name]
     ch = G.direct_ychunks(name, r.n, 1)
     assert ch

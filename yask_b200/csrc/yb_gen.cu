@@ -78,9 +78,11 @@ struct GenEngine : Engine {
         for (auto& kv : sweep_maps) cudaFree(kv.second);
         sweep_maps.clear();
     }
-    bool wide = false;   // kernels in their 64-bit addressing form (prepare)
+    bool wide = false;   // kernels in their 64-bit addressing form (prepare); option gen_wide reads it back
+    bool force_wide = false;   // option gen_wide = 1: the 64-bit form at any size (0: only where a slot needs it)
     int l2_mb = 16;    // option gen_l2_mb (env YB_GEN_L2_MB): L2 budget of one y chunk's sweep working set (0 = no chunking)
     int set_option(Solution&, const std::string& key, const std::string& value) override {
+        if (key == "gen_wide") { force_wide = atoi(value.c_str()) != 0; return 0; }
         if (key == "gen_pf") { pf_dist = std::max(0, atoi(value.c_str())); return 0; }
         if (key == "gen_l2_mb") { l2_mb = std::max(0, atoi(value.c_str())); return 0; }
         if (key == "gen_sweep") { sweep = atoi(value.c_str()) != 0; return 0; }
@@ -93,8 +95,9 @@ struct GenEngine : Engine {
         if (s.spec.elem_bytes != g.elem_bytes)
             return set_error(YB_EUNSUPPORTED, "solution '%s' was generated for %d-byte elements", g.name.c_str(), g.elem_bytes);
         // the kernels' addressing form (GenFnPair): 64-bit element positions once a var slot holds 2^31 elements or
-        // more, the 32-bit form below that (scratch vars share the solution's geometry, so the API-visible vars decide)
-        wide = false;
+        // more, the 32-bit form below that (scratch vars share the solution's geometry, so the API-visible vars decide);
+        // option gen_wide = 1 takes the 64-bit form at any size, so that it can be checked on small domains
+        wide = force_wide;
         for (auto& v : s.vars) wide = wide || v.slot_elems >= (int64_t(1) << 31);
         sweep_launches = 0;
         for (auto& st : g.stages)
@@ -171,8 +174,10 @@ struct GenEngine : Engine {
         return 0;
     }
     // Read-only option gen_sweep_launches: sweep-kernel launches since prepare (which parts took the TMA sweep form).
+    // Option gen_wide on a prepared solution: the addressing form its kernels run, "1" (64-bit) or "0" (32-bit).
     int64_t sweep_launches = 0;
-    bool get_option(const Solution&, const std::string& key, std::string& v) const override {
+    bool get_option(const Solution& s, const std::string& key, std::string& v) const override {
+        if (key == "gen_wide" && s.prepared) { v = wide ? "1" : "0"; return true; }
         if (key != "gen_sweep_launches") return false;
         v = std::to_string(sweep_launches);
         return true;
